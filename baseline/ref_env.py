@@ -8,7 +8,7 @@ box).  ``activate()`` puts it on ``sys.path`` and stubs the two pure-Python depe
 SURVEY.md Appendix D.
 
 ``use_prebuilt_extensions()`` hands the reference's loader (``quantization/extensions.py:28-72``) the
-reference's own CUDA extensions, compiled ahead of time for sm_100a from the reference sources by
+reference's own CUDA extensions, compiled ahead of time for sm_90a from the reference sources by
 ``oracle/build_ref_ext.py`` with the flags the loader itself uses.  It only skips the JIT compile (minutes per
 translation unit on a fresh box); the code that runs is the reference's.
 """

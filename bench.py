@@ -10,7 +10,7 @@ fixed model): the ranks form a pipeline -- every step a rank receives the hidden
 from rank - 1 and sends its own to rank + 1 (NCCL point-to-point over NVLink, overlapped with the kernels) -- and
 the only collective is ONE all-reduce(MAX) of the amax arena per calibration job (the timed K steps are one job).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Prints one JSON line (rank 0).  See DESIGN.md "Measurement" for every key.
 """
@@ -55,7 +55,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data-sheet HBM3 bandwidth, not a measurement)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -313,7 +313,7 @@ def _event_ms(fn, reps, dev):
 
 def north_star_4096(dev, peak):
     """The north-star tensor alone: per-tensor amax collect and NVFP4 fake quant of ONE 4096 x 4096 bf16 tensor per
-    launch, CUDA-event timed over a rotation of 16 distinct inputs (512 MiB >> 126 MB L2) replayed from a CUDA
+    launch, CUDA-event timed over a rotation of 16 distinct inputs (512 MiB >> 50 MB L2) replayed from a CUDA
     graph (launch-latency free, like the step); plus the grouped (pointer-array) launch over the same 16."""
     import torch
 
@@ -431,7 +431,7 @@ def run_gpu(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a CUDA device: the b200 engine has no CPU fallback")
+        raise SystemExit("bench.py needs a CUDA device: the engine has no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -499,6 +499,8 @@ def run_gpu(args):
     sampler = ClockSampler(local) if rank == 0 else None
     ms_step, (t_wall0, t_wall1) = timed_job(eng, args.steps, max(args.warmup, 3), sampler)
     clocks = sampler.stop(t_wall0, t_wall1) if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, acts, outs, args.dump_outputs)     # before anything below reuses the buffers
     value = TOKENS / (ms_step * 1e-3)
     comm_counts = dict(eng.comm_log)
 
@@ -649,6 +651,30 @@ def run_gpu(args):
         dist.destroy_process_group()
 
 
+DUMP_SAMPLE = 1 << 20      # elements kept per fake-quant output: 4 MiB as float32
+
+
+def dump_outputs(eng, acts, outs, dirpath):
+    """What the last timed step handed to its caller, as float32 .npy files: ``amax.npy`` (the calibrated amax of
+    every quantizer, in arena order) and, for the quantizers whose fake-quant output is still in the output ring
+    (the last ``len(outs)``), ``<name>.npy``: the elements at the sorted distinct values of ``DUMP_SAMPLE`` flat
+    indices drawn by ``torch.randint`` from a CPU generator seeded with 0, the same on every run.  One GPU only: with
+    the pipeline hand-off, a rank's last o_proj output goes to the hand-off buffer instead of the ring."""
+    import numpy as np
+    import torch
+
+    torch.cuda.synchronize(eng.device)
+    os.makedirs(dirpath, exist_ok=True)
+    np.save(os.path.join(dirpath, "amax.npy"), eng.amax_arena.float().cpu().numpy())
+    n = len(outs)
+    g = torch.Generator().manual_seed(0)
+    for i in range(max(0, len(eng.quantizers) - n), len(eng.quantizers)):
+        name = eng.quantizers[i][0]
+        y = outs[i % n][: acts[i].numel()]
+        idx = torch.randint(0, y.numel(), (DUMP_SAMPLE,), generator=g).unique()
+        np.save(os.path.join(dirpath, f"{name}.npy"), y[idx.to(y.device)].float().cpu().numpy())
+
+
 def run_e2e(eng, acts, outs, dev, world, args, barrier):
     """Same step through the engine API with HOST buffers: every step copies each quantizer's
     activation from pinned host memory into its device buffer (copy stream, overlapped with the collect
@@ -713,6 +739,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (amax + fake-quant samples) as .npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-config5", action="store_true", help="skip the Llama-3-70B extra of an 8-GPU run")
     ap.add_argument("--llama-ptq", type=int, default=32, metavar="LAYERS",
@@ -721,6 +749,10 @@ def main():
     ap.add_argument("--model", default="llama-3-8b", choices=["llama-3-8b", "llama-3-70b"],
                     help="shape plan; the default is the BASELINE metric's model (70b = BASELINE config 5)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.gpus > 1 or int(os.environ.get("WORLD_SIZE", "1")) > 1):
+        ap.error("--dump-outputs needs --gpus 1")
     if args.impl == "reference":
         run_reference(args)
     else:

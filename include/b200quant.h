@@ -1,5 +1,5 @@
 /*
- * b200quant.h -- C-ABI of the B200-native PTQ calibration / fake-quant / quant-and-pack engine.
+ * b200quant.h -- C-ABI of the H100-native PTQ calibration / fake-quant / quant-and-pack engine.
  *
  * This header is the drop-in boundary for the hot path named in BASELINE.json: every entry point
  * is what a binding of NVIDIA/Model-Optimizer's quantization extension modules would call.  Each

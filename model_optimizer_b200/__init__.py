@@ -1,4 +1,4 @@
-"""model_optimizer_b200 -- a B200-native (sm_100a) PTQ calibration / fake-quant / quant-and-pack
+"""model_optimizer_b200 -- a H100-native (sm_90a) PTQ calibration / fake-quant / quant-and-pack
 engine behind the ``modelopt.torch.quantization`` API surface.
 
 Layout: ``csrc/`` hand-written CUDA + the C-ABI (``include/b200quant.h``), ``_lib``/``ops`` the

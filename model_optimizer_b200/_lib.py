@@ -2,7 +2,7 @@
 
 The product path has NO CPU fallback: if the shared library is missing or a call fails, an
 exception is raised.  The library is built in-tree by ``__graft_entry__.build()`` (plain nvcc,
-sm_100a only) into ``model_optimizer_b200/lib/libb200quant.so``.
+sm_90a only) into ``model_optimizer_b200/lib/libb200quant.so``.
 """
 
 from __future__ import annotations

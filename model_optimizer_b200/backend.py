@@ -2,7 +2,7 @@
 SURVEY.md 8(b), plus the three module-level functions the hooks cannot reach.
 
 1. ``register_quant_backend("b200", entrypoint)`` (nn/modules/tensor_quantizer.py:87-109): fake quant of
-   any quantizer whose config carries ``backend: "b200"`` runs the fused sm_100a kernels.
+   any quantizer whose config carries ``backend: "b200"`` runs the fused sm_90a kernels.
 2. ``calibrator`` config field (config.py:599-614): ``B200MaxCalibrator`` / ``B200HistogramCalibrator``
    subclass the reference's ``_Calibrator`` so ``TensorQuantizer.collect`` reaches the collect kernels.
 3. ``_register_fp8_sweep_calibrator("b200", factory)`` (model_calib.py:166-179): the per-block FP8-scale
@@ -145,7 +145,7 @@ def make_cuda_ext_mx() -> types.SimpleNamespace:
         if int(format) == Types.E2M1 and int(scale_format) == Types.E4M3 and global_amax is not None \
                 and block_size == 16:
             return ops.fake_quant_nvfp4(x, global_amax.float().amax() if global_amax.numel() > 1 else global_amax)
-        raise NotImplementedError("fused_amax_convert: the B200 engine covers E8M0 scales and NVFP4 (E2M1 / E4M3)")
+        raise NotImplementedError("fused_amax_convert: the b200quant engine covers E8M0 scales and NVFP4 (E2M1 / E4M3)")
 
     return types.SimpleNamespace(fused_amax_convert=fused_amax_convert, convert_to_exmy=ops.convert_to_exmy,
                                  Types=Types)

@@ -1,4 +1,4 @@
-"""Calibrators -- the B200 counterpart of ``modelopt/torch/quantization/calib``.
+"""Calibrators -- the b200quant counterpart of ``modelopt/torch/quantization/calib``.
 
 ``collect`` is one fused kernel per batch (|x| max / histogram folded into device-resident fp32
 state); nothing synchronises with the host until ``compute_amax``."""

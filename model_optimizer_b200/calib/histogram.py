@@ -1,4 +1,4 @@
-"""HistogramCalibrator on the B200 engine.
+"""HistogramCalibrator on the b200quant engine.
 
 Reference: ``modelopt/torch/quantization/calib/histogram.py:35-343``.  ``collect`` in the reference
 is ``min()`` (sync) -> ``abs()`` -> ``float()`` -> ``max()`` -> ``histc`` (4-5 passes, fp32 copy);

@@ -1,4 +1,4 @@
-"""MaxCalibrator on the B200 engine.
+"""MaxCalibrator on the b200quant engine.
 
 Reference: ``modelopt/torch/quantization/calib/max.py:26-94`` -- ``collect`` computes
 ``reduce_amax(x, axis)`` (two full ATen reductions + abs/maximum) and keeps the running elementwise

@@ -1,4 +1,4 @@
-"""MseCalibrator on the B200 engine.
+"""MseCalibrator on the b200quant engine.
 
 Reference: ``modelopt/torch/quantization/calib/mse.py:31-172``.  Its ``collect`` runs, for each of the
 ``ceil((stop - start) / step) + 1`` multipliers, a full fake quant of the fp32 copy of the tensor, a squared-error

@@ -1,4 +1,4 @@
-"""NVFP4ActHeadroomCalibrator on the B200 engine.
+"""NVFP4ActHeadroomCalibrator on the b200quant engine.
 
 Reference: ``modelopt/torch/quantization/calib/nvfp4_act_headroom.py:36-205`` -- ``collect`` is a clone +
 two reductions (per-block amax) + boolean-mask compaction (a host sync) + log2 + bincount per batch; here it

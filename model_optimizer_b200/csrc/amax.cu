@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(kThreads)
 // per-tensor, TMA variant: persistent CTAs stream 16-32 KB tiles through a shared-memory ring with
 // cp.async.bulk (UBLKCP) + mbarrier transaction counts; one elected thread issues the copies, all
 // threads reduce from shared memory.  Selected with the "amax_tma" tuning knob (see DESIGN.md 5 for
-// the measured comparison with the LDG.E.256 kernel above).
+// its comparison with the vector-load kernel above).
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {

@@ -16,7 +16,7 @@
 namespace b200q {
 
 constexpr int kHistThreads = 512;          // block_log2_hist_kernel
-// histogram_kernel, two layouts of the CTA-private counters (knob "hist_variant"; both measured in profiles/):
+// histogram_kernel, two layouts of the CTA-private counters (knob "hist_variant"):
 //   single copy  : one u32 counter per bin (bins < kHsBins), 512 threads, several CTAs per SM
 //   lane private : 32 u16 copies of bins < kHcPriv, lane L only ever touches bank L (no bank conflicts), 1024 threads
 constexpr int kHsBins = 8192;
@@ -194,7 +194,7 @@ constexpr int kPatterns = 32768;
 
 // Generic form (fp16, and bf16 with knob hist_hot=0): one CTA-private u32[32768] table.  32 random addresses cost ~3.4
 // shared-memory wavefronts per warp instruction (bank conflicts), and RED.shared retires about one wavefront per 2.3
-// cycles per SM (profiles/r02_ncu_pattern_multi.txt) -- that, not HBM, bounds this form.
+// cycles per SM -- that, not HBM, bounds this form.
 template <typename Tag>
 __global__ void __launch_bounds__(kPatThreads, 1)
     hist_pattern_count_kernel(const uint8_t *__restrict__ x, size_t head, size_t nvec, size_t tail,
@@ -383,8 +383,8 @@ __global__ void __launch_bounds__(kPatThreads, 1)
   if (threadIdx.x == 0 && s_low) atomicAdd(scratch, s_low);  // credited to pattern 0 (value 0 -> bin 0)
   // flush: thread t sums the 32 lane copies of patterns t, t + 1024 (rotated 16-byte reads: conflict-free) and STORES the
   // totals into this CTA's own row of the global scratch -- no atomics; the bin kernel adds the rows up.  (The first
-  // version flushed with one global atomic per (CTA, pattern): 148 CTAs hammering the same 1536 addresses in the same
-  // order took 60 % of the kernel, profiles/r02_ncu_pattern_hot.txt.)
+  // version flushed with one global atomic per (CTA, pattern): 132 CTAs hammering the same 1536 addresses in the same
+  // order took 60 % of the kernel.)
   uint32_t *row = scratch + kPatterns + (size_t)blockIdx.x * kHot;
   for (int d = threadIdx.x; d < kHot; d += kPatThreads) {
     const uint4 *q = reinterpret_cast<const uint4 *>(s_pat + d * 32);

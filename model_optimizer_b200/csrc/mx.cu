@@ -7,10 +7,10 @@
 //   MXFP8 pack : quantization/qtensor/mxfp8_tensor.py:42-65, 150-262
 //   MXFP4 pack : quantization/qtensor/mxfp4_tensor.py:37-144
 //
-// One thread owns one block: for 16-bit inputs a 32-element block is two 32-byte LDG.E.256, the
+// One thread owns one block: for 16-bit inputs a 32-element block is two 32-byte vectors (four LDG.E.128), the
 // block amax is an in-register packed-integer max, the scale is an exponent read off the bits of
 // one IEEE division, and because the scale is a power of two the element path is
-// mul -> hardware narrow-format cvt (RNE, satfinite) -> cvt back -> mul, sign OR-ed back on the
+// mul -> narrow-format rounding (RNE, satfinite) -> back to float -> mul, sign OR-ed back on the
 // packed words.  The reference spends one thread per ELEMENT with a cub reduction per block.
 //
 // Conventions fixed here where the reference leaves them open (its `sign` variable is
@@ -58,7 +58,7 @@ __device__ __forceinline__ int e8m0_exponent_nv(float amax, float dmax) {
   return up ? ex - 126 : ex - 127;
 }
 
-// ---- element rounding of non-negative magnitudes (pairs, so the packed hardware cvt is used) ----
+// ---- element rounding of non-negative magnitudes (pairs, so the packed FP8 cvt is used) ----
 template <int FMT> struct MxRound;
 
 template <> struct MxRound<kE4M3> {
@@ -78,29 +78,20 @@ template <> struct MxRound<kE5M2> {
 };
 template <> struct MxRound<kE2M1> {
   static __device__ __forceinline__ void pair(float a0, float a1, float &r0, float &r1) {
-    const uint32_t h2 = e2m1x2_to_f16x2(f32x2_to_e2m1x2(a0, a1));
-    r0 = h2f_bits((uint16_t)(h2 & 0xffffu));
-    r1 = h2f_bits((uint16_t)(h2 >> 16));
+    r0 = e2m1_round_mag(a0);
+    r1 = e2m1_round_mag(a1);
   }
 };
-template <> struct MxRound<kE3M2> {
+template <> struct MxRound<kE3M2> {  // bias 3: minimum normal exponent -2, max 28
   static __device__ __forceinline__ void pair(float a0, float a1, float &r0, float &r1) {
-    uint16_t p;
-    uint32_t h2;
-    asm("cvt.rn.satfinite.e3m2x2.f32 %0, %1, %2;" : "=h"(p) : "f"(a1), "f"(a0));
-    asm("cvt.rn.f16x2.e3m2x2 %0, %1;" : "=r"(h2) : "h"(p));
-    r0 = h2f_bits((uint16_t)(h2 & 0xffffu));
-    r1 = h2f_bits((uint16_t)(h2 >> 16));
+    r0 = minifloat_rne_sat<2, -2>(a0, 28.f);
+    r1 = minifloat_rne_sat<2, -2>(a1, 28.f);
   }
 };
-template <> struct MxRound<kE2M3> {
+template <> struct MxRound<kE2M3> {  // bias 1: minimum normal exponent 0, max 7.5
   static __device__ __forceinline__ void pair(float a0, float a1, float &r0, float &r1) {
-    uint16_t p;
-    uint32_t h2;
-    asm("cvt.rn.satfinite.e2m3x2.f32 %0, %1, %2;" : "=h"(p) : "f"(a1), "f"(a0));
-    asm("cvt.rn.f16x2.e2m3x2 %0, %1;" : "=r"(h2) : "h"(p));
-    r0 = h2f_bits((uint16_t)(h2 & 0xffffu));
-    r1 = h2f_bits((uint16_t)(h2 >> 16));
+    r0 = minifloat_rne_sat<3, 0>(a0, 7.5f);
+    r1 = minifloat_rne_sat<3, 0>(a1, 7.5f);
   }
 };
 template <> struct MxRound<kINT8> {  // rint + clamp (tensor_quant_mx.h:84-93)

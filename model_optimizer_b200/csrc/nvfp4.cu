@@ -1,11 +1,11 @@
 // nvfp4.cu -- NVFP4 (E2M1 values, E4M3 scale per 16-element block, fp32 per-tensor scale):
 // dynamic / static fake quant, quant-and-pack, unpack.
 //
-// One thread owns one 16-element block: a single 32-byte LDG.E.256 brings the block into
+// One thread owns one 16-element block: one 32-byte vector (two LDG.E.128) brings the block into
 // registers, the block amax is an in-register packed-integer max (no shuffles), the two-level
-// scale is computed once per block, E2M1 rounding uses the Blackwell cvt.rn.satfinite.e2m1x2.f32
-// instruction (exactly the round-to-nearest-even table of the reference), and the block leaves
-// with one STG.E.256 (fake quant) or one 8-byte + one 1-byte store (pack).
+// scale is computed once per block, E2M1 rounding is the round-to-nearest-even table of the
+// reference (e2m1_round_mag / f32x2_to_e2m1x2 in common.cuh: sm_90 has no FP4 convert), and the block leaves with
+// one 32-byte vector store (fake quant) or one 8-byte + one 1-byte store (pack).
 //
 // Reference semantics:
 //   dynamic fake quant : kernels/quantization/gemm/fp4_kernel_hopper.py:33-170 +
@@ -19,21 +19,8 @@ namespace b200q {
 
 constexpr int kNvThreads = 256;
 
-// E2M1 round-to-nearest-even of a non-negative magnitude, written like the reference's
-// compare chain (common/nvfp4_quant.py:33-60); used on the slow path only.
-__device__ __forceinline__ float e2m1_round_mag(float a) {
-  return a <= 0.25f ? 0.0f
-         : a < 0.75f ? 0.5f
-         : a <= 1.25f ? 1.0f
-         : a < 1.75f ? 1.5f
-         : a <= 2.5f ? 2.0f
-         : a < 3.5f ? 3.0f
-         : a <= 5.0f ? 4.0f
-                     : 6.0f;
-}
-
 // out = sign(x) * e2m1(|x| / s) * s for the 16 elements of a block (s > 0).
-// fast path: hoisted exact division + hardware E2M1 conversion, sign OR-ed back on the packed
+// fast path: hoisted exact division + E2M1 rounding of the magnitude, sign OR-ed back on the packed
 // words; slow path (non-finite block, scale outside the safe exponent window): reference order.
 template <typename Tag, int VB>
 __device__ __forceinline__ void qdq_block(Block<Tag, VB> &b, float s, bool finite) {
@@ -52,9 +39,8 @@ __device__ __forceinline__ void qdq_block(Block<Tag, VB> &b, float s, bool finit
         const float q0 = __fmul_rn(lo, d.y), q1 = __fmul_rn(hi, d.y);
         const float t0 = __fmaf_rn(q0, -s, lo), t1 = __fmaf_rn(q1, -s, hi);
         const float a0 = __fmaf_rn(d.y, t0, q0), a1 = __fmaf_rn(d.y, t1, q1);
-        const uint32_t h2 = e2m1x2_to_f16x2(f32x2_to_e2m1x2(a0, a1));
-        const float r0 = __fmul_rn(h2f_bits((uint16_t)(h2 & 0xffffu)), s);
-        const float r1 = __fmul_rn(h2f_bits((uint16_t)(h2 >> 16)), s);
+        const float r0 = __fmul_rn(e2m1_round_mag(a0), s);
+        const float r1 = __fmul_rn(e2m1_round_mag(a1), s);
         b.word(i) = Elem<Tag>::pack(r0, r1) | (w & Elem<Tag>::NEG_ZERO2);
       }
     } else {
@@ -65,9 +51,8 @@ __device__ __forceinline__ void qdq_block(Block<Tag, VB> &b, float s, bool finit
         const float q0 = __fmul_rn(lo, d.y), q1 = __fmul_rn(hi, d.y);
         const float t0 = __fmaf_rn(q0, -s, lo), t1 = __fmaf_rn(q1, -s, hi);
         const float a0 = __fmaf_rn(d.y, t0, q0), a1 = __fmaf_rn(d.y, t1, q1);
-        const uint32_t h2 = e2m1x2_to_f16x2(f32x2_to_e2m1x2(a0, a1));
-        const float r0 = __fmul_rn(h2f_bits((uint16_t)(h2 & 0xffffu)), s);
-        const float r1 = __fmul_rn(h2f_bits((uint16_t)(h2 >> 16)), s);
+        const float r0 = __fmul_rn(e2m1_round_mag(a0), s);
+        const float r1 = __fmul_rn(e2m1_round_mag(a1), s);
         b.word(i) = __float_as_uint(r0) | (w0 & 0x80000000u);
         b.word(i + 1) = __float_as_uint(r1) | (w1 & 0x80000000u);
       }
@@ -141,7 +126,7 @@ __global__ void __launch_bounds__(kNvThreads)
 
 // TMA-store variant (north-star "TMA bulk staging" on the WRITE side; knob "nvfp4_tma_store"): the CTA's 16 KB of
 // results are staged in shared memory and leave as ONE cp.async.bulk.global.shared::cta (UBLKCP) issued by an elected
-// thread instead of 512 STG.E.256.  Bit-identical; measured against the STG kernel in profiles/ (DESIGN.md section 3).
+// thread instead of 512 32-byte vector stores.  Bit-identical to the STG kernel.
 template <typename Tag, int UNROLL>
 __global__ void __launch_bounds__(kNvThreads)
     nvfp4_dyn_tma_store_kernel(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t n_blocks,

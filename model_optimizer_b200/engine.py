@@ -127,7 +127,7 @@ class ShardedPTQEngine:
             # that stores into the next rank's inbox over NVLink / NVSwitch peer memory (full link bandwidth at
             # any world size) bracketed by two device-side barriers, instead of an NCCL send / recv pair (whose
             # point-to-point channel count shrinks with the communicator size: 415 GB/s at N = 2 but 81 GB/s at
-            # N = 8, profiles/r02_bench_n8.json).  Setup failure -> the NCCL path below.
+            # N = 8).  Setup failure -> the NCCL path below.
             self._symm = None
             self._peer_in = None
             self.handoff_transport = "nccl send/recv"

@@ -5,7 +5,7 @@ static block reshape :975-1061, ``load_calib_amax`` :697-720, ``export_amax`` :1
 
 Same attribute names and state (``_amax`` buffer in the input dtype, ``_pre_quant_scale``,
 ``_if_quant`` / ``_if_calib`` / ``_disabled``), same dispatch rules; every numeric step is a
-fused sm_100a kernel (``model_optimizer_b200.ops``).  CPU tensors raise.
+fused sm_90a kernel (``model_optimizer_b200.ops``).  CPU tensors raise.
 """
 
 from __future__ import annotations
@@ -477,7 +477,13 @@ class TensorQuantizer(nn.Module):
                                  "Expected (2, 1) for MXFP4 or (4, 3) for MXFP8.")
             self._scale = sc
         elif self._num_bits == (2, 1):
-            q, sf, sf2 = NVFP4QTensor.quantize(inputs, bs[-1])
+            # second-level scale from the calibration when there is one (tensor_quantizer.py:867-875,
+            # NVFP4QTensor.get_weights_scaling_factor_2_from_quantizer): the static global amax, else _amax
+            wsf2 = None
+            if self.amax is not None:
+                g = getattr(self, "_global_amax", None) if self.is_static_block_quant else None
+                wsf2 = (g if g is not None else self._amax).float() / (6.0 * 448.0)
+            q, sf, sf2 = NVFP4QTensor.quantize(inputs, bs[-1], weights_scaling_factor_2=wsf2)
             self._scale, self._double_scale = sf, sf2
         elif bs and bs.get("scale_bits", 0) == 8 and bs.get("scale_block_sizes"):
             # NF4 with double quantization of the scales (tensor_quantizer.py:841-856)
@@ -489,7 +495,11 @@ class TensorQuantizer(nn.Module):
             q, sc = INT4QTensor.quantize(inputs, bs[-1])
             self._scale = sc
         elif self._num_bits == (4, 3):
-            q, sc = FP8QTensor.quantize(inputs, axis=self._axis)
+            # per-tensor / per-channel scales from the calibrated amax (:824-835); 2-D blocks recompute theirs from
+            # the weight, which gives the reference's packs and scales bit for bit after max calibration
+            use_amax = self.amax is not None and not bs
+            q, sc = FP8QTensor.quantize(inputs, axis=self._axis, block_sizes=bs or None,
+                                        scales=self.amax / 448.0 if use_amax else None)
             self._scale = sc
         else:
             raise NotImplementedError(f"real quantization for num_bits={self._num_bits}")

@@ -1,6 +1,6 @@
-"""Tensor quantization functionals -- the B200 counterpart of
+"""Tensor quantization functionals -- the b200quant counterpart of
 ``modelopt/torch/quantization/tensor_quant.py``: same names, same argument meaning, every forward
-is ONE fused sm_100a kernel reached through the C-ABI; backward is the reference's straight-through
+is ONE fused sm_90a kernel reached through the C-ABI; backward is the reference's straight-through
 estimator with the ``|x| <= amax`` clip (tensor_quant.py:290-316)."""
 
 from __future__ import annotations
@@ -119,7 +119,7 @@ class DynamicBlockQuantizationFunction(Function):
             return ops.fake_quant_mx(inputs.contiguous(), block_size, mx_format_map[num_bits])
         if num_bits != (2, 1) or scale_bits != (4, 3):
             raise NotImplementedError(
-                f"dynamic block quantization num_bits={num_bits} scale_bits={scale_bits}: the B200 engine has "
+                f"dynamic block quantization num_bits={num_bits} scale_bits={scale_bits}: the b200quant engine has "
                 "kernels for NVFP4 (E2M1 + E4M3 scales) and for E8M0-scaled MX formats")
         # like the reference's Triton branch (tensor_quant.py:175-183, fp4_kernel_hopper.py:102), the NVFP4
         # fake quant always works on 16-element blocks; block_size only matters to the pack / export path

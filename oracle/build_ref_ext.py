@@ -1,4 +1,4 @@
-"""Build the REFERENCE's own CUDA extensions for sm_100a from the sources where they lie
+"""Build the REFERENCE's own CUDA extensions for sm_90a from the sources where they lie
 (/root/reference/modelopt/torch/kernels/quantization/gemm) into oracle/_ref/ -- nothing is copied into
 the repo.  Same source lists and extra flags as the reference's loader (quantization/extensions.py:28-72):
 
@@ -34,12 +34,13 @@ def build_one(name: str) -> str:
     srcs, flags = EXTS[name]
     dst = os.path.join(OUT, name + ".so")
     srcs = [os.path.join(SRC, s) for s in srcs]
-    if os.path.exists(dst) and all(os.path.getmtime(dst) >= os.path.getmtime(s) for s in srcs):
+    # this recipe (its gencode flags) is part of the key: a change of target architecture rebuilds
+    if os.path.exists(dst) and all(os.path.getmtime(dst) >= os.path.getmtime(s) for s in srcs + [__file__]):
         return dst
     bdir = os.path.join(OUT, "build_" + name)
     os.makedirs(bdir, exist_ok=True)
     cpp_extension.load(name=name, sources=srcs, build_directory=bdir, verbose=False, is_python_module=False,
-                       extra_cuda_cflags=["-gencode", "arch=compute_100a,code=sm_100a", *flags])
+                       extra_cuda_cflags=["-gencode", "arch=compute_90a,code=sm_90a", *flags])
     shutil.copyfile(os.path.join(bdir, name + ".so"), dst)
     shutil.rmtree(bdir, ignore_errors=True)
     return dst
@@ -49,7 +50,7 @@ def main() -> int:
     if not os.path.isdir(SRC):
         print("reference sources not present: nothing to build")
         return 0
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.makedirs(OUT, exist_ok=True)
     with ThreadPoolExecutor(3) as ex:
         for p in ex.map(build_one, EXTS):

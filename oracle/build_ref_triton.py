@@ -1,4 +1,4 @@
-"""AOT-compile the REFERENCE's Triton kernels for sm_100 into oracle/_ref/ (cubins + one JSON index).
+"""AOT-compile the REFERENCE's Triton kernels for sm_90 into oracle/_ref/ (cubins + one JSON index).
 
 The kernels are the reference's own ``@triton.jit`` functions, imported from /root/reference where they lie
 (nothing is copied into the repo) and compiled with the Triton that ships in this image -- no GPU needed:
@@ -47,7 +47,7 @@ def main() -> int:
     hopper = importlib.import_module(base + "fp4_kernel_hopper")
     fp4 = importlib.import_module(base + "fp4_kernel")
     sweep = importlib.import_module(base + "nvfp4_fp8_sweep")
-    target = GPUTarget("cuda", 100, 32)
+    target = GPUTarget("cuda", 90, 32)
     tdt = {"bf16": tl.bfloat16, "f16": tl.float16, "f32": tl.float32}
     ptr = {"bf16": "*bf16", "f16": "*fp16", "f32": "*fp32"}
     index = {"triton": triton.__version__, "kernels": {}}

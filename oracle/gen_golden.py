@@ -16,6 +16,11 @@ import types
 
 import numpy as np
 
+try:
+    from oracle import golden
+except ImportError:          # run as python oracle/gen_golden.py
+    import golden
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 OUT = os.path.join(ROOT, "tests", "golden")
 
@@ -191,8 +196,8 @@ def main():
                 out[f"{key}/hist2_edges_last"] = hc._calib_bin_edges[-1].numpy().copy()
 
     out["cases"] = np.array(cases)
-    np.savez_compressed(os.path.join(OUT, "ref_small.npz"), **out)
-    print("wrote", os.path.join(OUT, "ref_small.npz"), len(out), "arrays")
+    golden.save("ref_small", out, OUT)
+    print("wrote ref_small", len(out), "arrays")
 
 
 
@@ -427,8 +432,8 @@ def main_mx():
         out[f"qt/{dname}/ragged/mxfp8/q"] = q8._quantized_data.view(torch.uint8).numpy().copy()
         out[f"qt/{dname}/ragged/mxfp8/scale"] = s8.numpy().copy()
         out[f"qt/{dname}/ragged/mxfp8/deq"] = q8.dequantize(dtype=dt, scale=s8).float().numpy().view(np.uint32)
-    np.savez_compressed(os.path.join(OUT, "ref_mx.npz"), **out)
-    print("wrote", os.path.join(OUT, "ref_mx.npz"), len(out), "arrays")
+    golden.save("ref_mx", out, OUT)
+    print("wrote ref_mx", len(out), "arrays")
 
 
 def main_bias():
@@ -511,8 +516,8 @@ def main_fp8_blocks():
                 wsf = (tq.amax.float() / 448.0).squeeze()
                 q2, _ = FP8QTensor.quantize(x, wsf, block_sizes=dict(blocks))
                 out[key + "/q_export"] = q2._quantized_data.view(torch.uint8).numpy().copy()
-    np.savez_compressed(os.path.join(OUT, "ref_fp8_blocks.npz"), **out)
-    print("wrote", os.path.join(OUT, "ref_fp8_blocks.npz"), len(out), "arrays")
+    golden.save("ref_fp8_blocks", out, OUT)
+    print("wrote ref_fp8_blocks", len(out), "arrays")
 
 
 def main_int8():
@@ -758,8 +763,8 @@ def main_export():
                 out[f"{key}/meta/{k}"] = np.array(json.dumps([str(v.dtype), list(v.shape)]))
             out[f"{key}/cfg"] = np.array(json.dumps(json.load(open(os.path.join(d, "hf_quant_config.json")))))
         print("export", key, len(sd), "tensors", json.loads(str(out[f"{key}/cfg"]))["quantization"])
-    np.savez_compressed(os.path.join(OUT, "ref_export.npz"), **out)
-    print("wrote ref_export.npz", len(out), "arrays", os.path.getsize(os.path.join(OUT, "ref_export.npz")) >> 10, "KiB")
+    golden.save("ref_export", out, OUT)
+    print("wrote ref_export", len(out), "arrays")
 
 
 if __name__ == "__main__":

@@ -970,7 +970,7 @@ def unpack_mxfp4(packed, scale_bytes, block_size=32, dtype="bf16"):
 
 # ------------------------------------------------------------------------------------------------
 # (6) NF4 (CUDA-extension semantics; the reference's CPU fallback rounds the table to the tensor dtype
-#     and is a different function -- the GPU kernels are pinned against the compiled extension on the B200)
+#     and is a different function -- the GPU kernels are pinned against the compiled extension on the GPU)
 # ------------------------------------------------------------------------------------------------
 NF4_LUT = np.array([-1.0, -0.6962, -0.5251, -0.3949, -0.2844, -0.1848, -0.0911, 0.0, 0.0796, 0.1609, 0.2461,
                     0.3379, 0.4407, 0.5626, 0.7230, 1.0], dtype=F32)      # tensor_quant_gpu.cu:142-144

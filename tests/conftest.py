@@ -9,11 +9,11 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 @pytest.fixture(scope="session")
 def golden():
-    import numpy as np
+    from oracle import golden as _golden
 
-    return np.load(os.path.join(ROOT, "tests", "golden", "ref_small.npz"))
+    return _golden.load("ref_small")

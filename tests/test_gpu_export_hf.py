@@ -10,6 +10,8 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
+
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TD = {"torch.bfloat16": torch.bfloat16, "torch.float32": torch.float32, "torch.float16": torch.float16,
@@ -18,7 +20,7 @@ TD = {"torch.bfloat16": torch.bfloat16, "torch.float32": torch.float32, "torch.f
 
 @pytest.fixture(scope="module")
 def fx():
-    return np.load(os.path.join(ROOT, "tests", "golden", "ref_export.npz"))
+    return golden.load("ref_export")
 
 
 def build_calibrated(fx, key, preset):

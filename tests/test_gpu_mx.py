@@ -9,12 +9,13 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import golden
 from oracle import oracle_np as o
 
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-G = np.load(os.path.join(ROOT, "tests", "golden", "ref_mx.npz"))
+G = golden.load("ref_mx")
 TD = {"bf16": torch.bfloat16, "f16": torch.float16, "f32": torch.float32}
 FMT_NAMES = ["E4M3", "E5M2", "INT8", "E0M3", "E1M2", "E3M0", "E2M1", "E3M2", "E2M3"]
 

@@ -9,6 +9,7 @@ import pytest
 import torch
 from torch import nn
 
+from oracle import golden
 from oracle import oracle_np as o
 
 pytestmark = pytest.mark.gpu
@@ -597,7 +598,7 @@ def test_fp8_block_scales_eager_rule_and_2d_blocks(ops):
     from model_optimizer_b200.nn import TensorQuantizer
     from model_optimizer_b200.qtensor import FP8QTensor
 
-    G = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_fp8_blocks.npz"))
+    G = golden.load("ref_fp8_blocks")
     keys = sorted({k.rsplit("/x", 1)[0] for k in G.files if k.endswith("/x")})
     assert len(keys) == 12
     for key in keys:

@@ -1,4 +1,4 @@
-"""Side by side on the GPU: the REFERENCE's own CUDA extensions (built for sm_100a by oracle/build_ref_ext.py
+"""Side by side on the GPU: the REFERENCE's own CUDA extensions (built for sm_90a by oracle/build_ref_ext.py
 from the sources under /root/reference into oracle/_ref/*.so, which travel with the snapshot) against this
 engine's kernels, on the same seeded inputs.  This is what pins the paths the CPU cannot execute:
 

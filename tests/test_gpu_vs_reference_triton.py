@@ -1,4 +1,4 @@
-"""Side by side on the GPU: the REFERENCE's Triton kernels -- AOT-compiled for sm_100 by
+"""Side by side on the GPU: the REFERENCE's Triton kernels -- AOT-compiled for sm_90 by
 oracle/build_ref_triton.py from the @triton.jit functions under /root/reference into oracle/_ref/*.cubin
 (which travel with the snapshot) -- launched through the CUDA driver API next to this engine's kernels.
 

@@ -9,9 +9,10 @@ import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
+import golden  # noqa: E402
 import oracle_np as o  # noqa: E402
 
-G = np.load(os.path.join(ROOT, "tests", "golden", "ref_fp8_blocks.npz"))
+G = golden.load("ref_fp8_blocks")
 F32 = np.float32
 
 

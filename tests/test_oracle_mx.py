@@ -10,9 +10,10 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
+import golden  # noqa: E402
 import oracle_np as o  # noqa: E402
 
-G = np.load(os.path.join(ROOT, "tests", "golden", "ref_mx.npz"))
+G = golden.load("ref_mx")
 F32 = np.float32
 
 

@@ -106,7 +106,7 @@ def main():
     for shp in args.shapes.split(","):
         r, c = (int(v) for v in shp.split("x"))
         n = r * c
-        nbuf = max(4, int((768 << 20) / (n * 2)))  # >= 768 MiB of distinct inputs (L2 is 126 MB)
+        nbuf = max(4, int((768 << 20) / (n * 2)))  # >= 768 MiB of distinct inputs (L2 is 50 MB)
         xs = [torch.randn(r, c, device=dev).to(torch.bfloat16) for _ in range(nbuf)]
         ys = [torch.empty_like(xs[0]) for _ in range(min(nbuf, 8))]
         slot = torch.zeros(1, dtype=torch.float32, device=dev)

@@ -1,6 +1,6 @@
 """SASS evidence (no GPU needed): per-kernel opcode histogram of model_optimizer_b200/lib/libb200quant.so from
 `cuobjdump -sass`, written to profiles/.  The .so is git-ignored; this text is what the repo carries to show the
-Blackwell instruction mix (LDG.E.256 / STG.E.256, F2FP e2m1 / e4m3 converts, UBLKCP bulk copies, REDUX, RED/ATOMS).
+instruction mix (LDG.E.128 / STG.E.128, F2FP e4m3 converts, UBLKCP bulk copies, REDUX, RED/ATOMS).
 
 usage: python tools/sass_report.py [out.txt]"""
 import collections
@@ -34,7 +34,7 @@ def main():
     dm = subprocess.run(["c++filt", "-p"], input="\n".join(names), capture_output=True, text=True).stdout.splitlines()
     demangle = dict(zip(names, dm)) if len(dm) == len(names) else {n: n for n in names}
     total = collections.Counter()
-    lines = [f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)}  ({len(kernels)} sm_100a kernels)",
+    lines = [f"# cuobjdump -sass {os.path.relpath(LIB, ROOT)}  ({len(kernels)} sm_90a kernels)",
              "# per kernel: instruction count, then the memory / convert / reduction opcodes that characterise it", ""]
     for k, c in kernels.items():
         n = sum(c.values())
