@@ -379,6 +379,9 @@ int b200q_nvfp4_fp8_scale_sweep_hessian(const void *w, int dtype, size_t cout, s
 /* Checks the hoisted-reciprocal exact division against div.rn.f32 on n pseudo-random pairs
  * (seeded); returns the number of mismatches in *mismatches_host. */
 int b200q_selftest_fastdiv(uint64_t seed, size_t n, unsigned long long *mismatches_host);
+/* Checks the branch-free E2M1 rounding of the fake-quant kernels against the reference's compare chain on every
+ * non-negative fp32 bit pattern (finite, +inf and NaN); returns the number of mismatches in *mismatches_host. */
+int b200q_selftest_e2m1_round(unsigned long long *mismatches_host);
 
 #ifdef __cplusplus
 }

@@ -78,6 +78,7 @@ _SIGNATURES = {
     "b200q_nvfp4_fp8_scale_sweep_ex": [_P, c_int, c_size_t, _P, _P, c_int, _P, _P],
     "b200q_nvfp4_fp8_scale_sweep_hessian": [_P, c_int, c_size_t, c_size_t, _P, _P, c_int, _P, _P, _P],
     "b200q_selftest_fastdiv": [c_uint64, c_size_t, _P],
+    "b200q_selftest_e2m1_round": [_P],
 }
 
 EXPORTED_SYMBOLS = ("b200q_version", "b200q_last_error", "b200q_convert_to_exmy", *_SIGNATURES.keys())

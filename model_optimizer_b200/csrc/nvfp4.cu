@@ -3,8 +3,8 @@
 //
 // One thread owns one 16-element block: one 32-byte vector (two LDG.E.128) brings the block into
 // registers, the block amax is an in-register packed-integer max (no shuffles), the two-level
-// scale is computed once per block, E2M1 rounding is the round-to-nearest-even table of the
-// reference (e2m1_round_mag / f32x2_to_e2m1x2 in common.cuh: sm_90 has no FP4 convert), and the block leaves with
+// scale is computed once per block, E2M1 rounding is the reference's round-to-nearest-even, branch-free
+// (e2m1_round_mag / f32x2_to_e2m1x2 in common.cuh: sm_90 has no FP4 convert), and the block leaves with
 // one 32-byte vector store (fake quant) or one 8-byte + one 1-byte store (pack).
 //
 // Reference semantics:
@@ -62,7 +62,9 @@ __device__ __forceinline__ void qdq_block(Block<Tag, VB> &b, float s, bool finit
     b.to_floats(f);
 #pragma unroll
     for (int e = 0; e < kBlk; ++e) {
-      const float r = __fmul_rn(e2m1_round_mag(__fdiv_rn(fabsf(f[e]), s)), s);
+      // a negative static block scale gives negative quotients, which the reference's chain rounds to 0
+      const float q = __fdiv_rn(fabsf(f[e]), s);
+      const float r = __fmul_rn(q < 0.f ? 0.f : e2m1_round_mag(q), s);
       f[e] = (f[e] >= 0.f) ? r : -r;
     }
     if constexpr (Elem<Tag>::PER_WORD == 2) {

@@ -94,6 +94,15 @@ __global__ void fastdiv_selftest_kernel(uint64_t seed, size_t n, unsigned long l
   if (__float_as_uint(q1) != __float_as_uint(q2)) atomicAdd(mism, 1ull);
 }
 
+// ---- E2M1 rounding self test ---------------------------------------------------------------
+// one thread per non-negative fp32 bit pattern (every finite value, +inf and the NaNs): the branch-free
+// e2m1_round_mag against the reference's compare chain, bit for bit
+__global__ void e2m1_round_selftest_kernel(unsigned long long *mism) {
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+  const float a = __uint_as_float(u);
+  if (__float_as_uint(e2m1_round_mag(a)) != __float_as_uint(e2m1_round_mag_ref(a))) atomicAdd(mism, 1ull);
+}
+
 }  // namespace b200q
 
 using namespace b200q;
@@ -153,6 +162,22 @@ int b200q_selftest_fastdiv(uint64_t seed, size_t n, unsigned long long *mismatch
   const size_t blocks = (n + threads - 1) / threads;
   if (blocks > 0) fastdiv_selftest_kernel<<<(unsigned)blocks, threads>>>(seed, n, d);
   int rc = check_launch("fastdiv_selftest");
+  cudaMemcpy(mismatches_host, d, sizeof(*d), cudaMemcpyDeviceToHost);
+  cudaFree(d);
+  return rc;
+}
+
+int b200q_selftest_e2m1_round(unsigned long long *mismatches_host) {
+  B200Q_REQUIRE(mismatches_host != nullptr, "mismatches_host is null");
+  unsigned long long *d = nullptr;
+  if (cudaMalloc(&d, sizeof(*d)) != cudaSuccess) {
+    set_error("cudaMalloc failed");
+    return B200Q_ERR_CUDA;
+  }
+  cudaMemset(d, 0, sizeof(*d));
+  const int threads = 256;
+  e2m1_round_selftest_kernel<<<(1u << 31) / threads, threads>>>(d);  // 2^31 patterns: sign bit clear
+  int rc = check_launch("e2m1_round_selftest");
   cudaMemcpy(mismatches_host, d, sizeof(*d), cudaMemcpyDeviceToHost);
   cudaFree(d);
   return rc;

@@ -679,6 +679,14 @@ def selftest_fastdiv(seed: int, n: int) -> int:
     return int(m.value)
 
 
+def selftest_e2m1_round() -> int:
+    import ctypes
+
+    m = ctypes.c_ulonglong(0)
+    call("b200q_selftest_e2m1_round", ctypes.byref(m))
+    return int(m.value)
+
+
 def _on_tensor_device(fn):
     """The C-ABI launches on the calling thread's current device.  Every public op runs with the device of its
     first CUDA tensor argument current and restores the previous one afterwards (nothing is cached: torch's
@@ -700,7 +708,7 @@ def _on_tensor_device(fn):
 for _n, _f in list(globals().items()):
     if callable(_f) and not isinstance(_f, type) and getattr(_f, "__module__", None) == __name__ \
             and not _n.startswith("_") \
-            and _n not in ("selftest_fastdiv", "convert_to_exmy"):
+            and _n not in ("selftest_fastdiv", "selftest_e2m1_round", "convert_to_exmy"):
         globals()[_n] = _on_tensor_device(_f)
 
 __all__ = [n for n in dir() if not n.startswith("_") and n not in ("torch", "functools", "annotations")]
