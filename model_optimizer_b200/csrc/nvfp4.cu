@@ -168,12 +168,49 @@ __global__ void __launch_bounds__(kNvThreads)
   }
 }
 
+// dynamic fake quant of the blocks base + u * stride (u < UNROLL) that are below n.  COLLECT: also returns their |x|
+// max as raw magnitude bits in the element's own format -- what amax_tensor_multi_kernel reduces, NaN payload included
+// (the block scale is the same either way: a non-finite block max gives the 448 clamp whatever its payload); 0 otherwise.
+template <typename Tag, int VB, int UNROLL, bool COLLECT>
+__device__ __forceinline__ uint32_t dyn_fq_blocks(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t base,
+                                                  size_t stride, size_t n, const DynScale &ds, const ExactDiv &d6) {
+  Block<Tag, VB> b[UNROLL];
+#pragma unroll
+  for (int u = 0; u < UNROLL; ++u) {
+    const size_t i = base + (size_t)u * stride;
+    if (i < n) b[u].load(x, i);
+  }
+  uint32_t amax = 0;
+#pragma unroll
+  for (int u = 0; u < UNROLL; ++u) {
+    const size_t i = base + (size_t)u * stride;
+    if (i >= n) continue;
+    uint32_t mb;
+    if constexpr (COLLECT) {
+      const uint32_t nb = b[u].prep_and_absmax_native_bits();
+      amax = max(amax, nb);
+      mb = Elem<Tag>::absbits_to_f32bits(nb);
+    } else {
+      mb = b[u].prep_and_absmax_bits();
+    }
+    const bool finite = mb < 0x7f800000u;
+    const float s = ds.block_scale(__uint_as_float(mb), d6);
+    qdq_block<Tag, VB>(b[u], s, finite);
+    b[u].store(y, i);
+  }
+  return amax;
+}
+
 // the same kernel over a table of tensors (common.cuh MultiDesc): CTA -> (tensor, tile of 256 * UNROLL blocks);
-// each tensor's global amax is amax_base[slot] (the engine's flat _amax arena)
-template <typename Tag, int VB, int UNROLL>
-__global__ void __launch_bounds__(kNvThreads)
+// each tensor's global amax is amax_base[slot] (the engine's flat _amax arena).
+// COLLECT: the pass is also the calibration collect -- the CTA's |x| max goes into the fp32 slot slots[slot] exactly as
+// amax_tensor_multi_kernel puts it there (unsigned atomic max on the bit pattern, nothing for an all-zero tile), so the
+// slot ends bit-identical to that kernel's.  The atomic is skipped when the slot already holds at least that value:
+// slots only grow, so the skip is exact.
+template <typename Tag, int VB, int UNROLL, bool COLLECT>
+__global__ void __launch_bounds__(kNvThreads, !COLLECT ? 0 : std::is_same<Tag, BF16Tag>::value ? 5 : 4)
     nvfp4_dyn_multi_kernel(const MultiDesc *__restrict__ descs, int n_desc, const void *__restrict__ amax_base,
-                           int gamax_dtype) {
+                           int gamax_dtype, uint32_t *__restrict__ slots) {
   pdl_launch_dependents();
   pdl_wait();
   const MultiDesc d = descs[multi_find(descs, n_desc)];
@@ -181,22 +218,96 @@ __global__ void __launch_bounds__(kNvThreads)
   ds.setup(load_scalar(amax_base, gamax_dtype, (size_t)d.slot));
   const ExactDiv d6(ds.six_gs);
   const size_t base = (size_t)(blockIdx.x - d.first_cta) * (kNvThreads * UNROLL) + threadIdx.x;
-  Block<Tag, VB> b[UNROLL];
-#pragma unroll
-  for (int u = 0; u < UNROLL; ++u) {
-    const size_t i = base + (size_t)u * kNvThreads;
-    if (i < d.n_units) b[u].load(d.x, i);
+  const uint32_t m = dyn_fq_blocks<Tag, VB, UNROLL, COLLECT>(d.x, d.y, base, kNvThreads, d.n_units, ds, d6);
+  if constexpr (COLLECT) {
+    const uint32_t cm = block_max<kNvThreads>(m);
+    if (threadIdx.x == 0 && cm != 0u) {
+      const uint32_t fb = Elem<Tag>::absbits_to_f32bits(cm);
+      if (fb > __ldcg(slots + d.slot)) atomicMax(slots + d.slot, fb);
+    }
   }
-#pragma unroll
-  for (int u = 0; u < UNROLL; ++u) {
-    const size_t i = base + (size_t)u * kNvThreads;
-    if (i >= d.n_units) continue;
-    const uint32_t mb = b[u].prep_and_absmax_bits();
-    const bool finite = mb < 0x7f800000u;
-    const float s = ds.block_scale(__uint_as_float(mb), d6);
-    qdq_block<Tag, VB>(b[u], s, finite);
-    b[u].store(d.y, i);
+}
+
+// Exact fix-up after a speculative COLLECT pass (which quantized with the amax exported one step earlier): an entry
+// whose new exported amax -- its fp32 slot rounded to amax_dtype as amax_export_kernel rounds it -- differs in bits
+// from amax_base[slot] (what the pass used; the export has not run yet) is quantized again with the new amax.
+// live[2 i], live[2 i + 1] = (live_from, contested_to) of entry i (ops.live_block_ranges).  Only its live blocks
+// [live_from, n_units) are redone: the prefix below live_from is overwritten by later entries of the table that share
+// the output buffer, and the live ranges of different entries never overlap.  An unchanged entry still rewrites
+// [live_from, contested_to), the part of its live range that earlier entries write too: the pass runs them
+// concurrently, so their stores may have landed after its own.  Each buffer then ends as the sequential launches leave
+// it.  Persistent grid: every CTA checks the entries 256 at a time (one per thread) and grid-strides over the range
+// of each one that has work; redo_count gets one increment per changed entry.
+template <typename Tag, int VB, int UNROLL>
+__global__ void __launch_bounds__(kNvThreads)
+    nvfp4_dyn_multi_fixup_kernel(const MultiDesc *__restrict__ descs, const unsigned long long *__restrict__ live,
+                                 int n_desc, const uint32_t *__restrict__ slots, const void *__restrict__ amax_base,
+                                 int amax_dtype, int *__restrict__ redo_count) {
+  __shared__ uint32_t s_work[kNvThreads / 32];
+  __shared__ float s_amax[kNvThreads];
+  __shared__ unsigned long long s_end[kNvThreads];
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t stride = (size_t)gridDim.x * kNvThreads;
+  const size_t gtid = (size_t)blockIdx.x * kNvThreads + threadIdx.x;
+  for (int e0 = 0; e0 < n_desc; e0 += kNvThreads) {
+    const int e = e0 + (int)threadIdx.x;
+    bool work = false;
+    if (e < n_desc) {
+      const long long slot = descs[e].slot;
+      const float v = __uint_as_float(__ldcg(slots + slot));
+      uint32_t nb, ob;
+      float na;
+      if (amax_dtype == B200Q_F32) {
+        nb = __float_as_uint(v);
+        ob = static_cast<const uint32_t *>(amax_base)[slot];
+        na = v;
+      } else if (amax_dtype == B200Q_BF16) {
+        nb = f2bf_bits(v);
+        ob = static_cast<const uint16_t *>(amax_base)[slot];
+        na = __uint_as_float(nb << 16);
+      } else {
+        nb = f2h_bits(v);
+        ob = static_cast<const uint16_t *>(amax_base)[slot];
+        na = h2f_bits((uint16_t)nb);
+      }
+      const bool redo = nb != ob;
+      const unsigned long long end = redo ? descs[e].n_units : live[2 * e + 1];
+      work = end > live[2 * e];
+      s_amax[threadIdx.x] = na;
+      s_end[threadIdx.x] = end;
+      if (redo && blockIdx.x == 0) atomicAdd(redo_count, 1);
+    }
+    const uint32_t ballot = __ballot_sync(0xffffffffu, work);
+    if ((threadIdx.x & 31) == 0) s_work[threadIdx.x >> 5] = ballot;
+    __syncthreads();
+    for (int w = 0; w < kNvThreads / 32; ++w) {
+      for (uint32_t bits = s_work[w]; bits != 0u; bits &= bits - 1u) {
+        const int k = w * 32 + __ffs((int)bits) - 1;
+        const MultiDesc d = descs[e0 + k];
+        const size_t end = s_end[k];
+        DynScale ds;
+        ds.setup(s_amax[k]);
+        const ExactDiv d6(ds.six_gs);
+        for (size_t i = live[2 * (e0 + k)] + gtid; i < end; i += stride * UNROLL)
+          dyn_fq_blocks<Tag, VB, UNROLL, false>(d.x, d.y, i, stride, end, ds, d6);
+      }
+    }
+    __syncthreads();  // s_work / s_amax / s_end are refilled for the next 256 entries
   }
+}
+
+template <typename Tag>
+static int launch_nvfp4_fixup(const MultiDesc *d, const unsigned long long *live, int n_desc, const uint32_t *slots,
+                              const void *amax_base, int amax_dtype, int *redo_count, cudaStream_t st) {
+  auto kern = nvfp4_dyn_multi_fixup_kernel<Tag, 32, 2>;
+  static int per_sm = 0;  // resident CTAs per SM: the grid is exactly one wave, so no CTA waits for another to finish
+  if (per_sm == 0 && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kNvThreads, 0) != cudaSuccess)
+    return check_launch("nvfp4_dyn_multi_fixup_kernel occupancy");
+  const int grid = sm_count() * (per_sm < 1 ? 1 : per_sm);
+  launch_pdl(kern, dim3((unsigned)grid), dim3(kNvThreads), 0, st, d, live, n_desc, slots, amax_base, amax_dtype,
+             redo_count);
+  return check_launch("nvfp4_dyn_multi_fixup_kernel");
 }
 
 // ragged rows (row_len % 16 != 0) or unaligned tensors: one thread per (row, block), scalar I/O
@@ -580,9 +691,40 @@ int b200q_fake_quant_nvfp4_multi(const void *descs, int n_desc, size_t total_cta
   B200Q_REQUIRE(total_ctas <= 0x7fffffffu, "too many CTAs");
   const MultiDesc *d = static_cast<const MultiDesc *>(descs);
   B200Q_DISPATCH_DTYPE(dtype, Tag,
-                       launch_pdl(nvfp4_dyn_multi_kernel<Tag, 32, 2>, dim3((unsigned)total_ctas), dim3(kNvThreads), 0,
-                                  (cudaStream_t)stream, d, n_desc, amax_base, amax_dtype));
+                       launch_pdl(nvfp4_dyn_multi_kernel<Tag, 32, 2, false>, dim3((unsigned)total_ctas), dim3(kNvThreads),
+                                  0, (cudaStream_t)stream, d, n_desc, amax_base, amax_dtype, nullptr));
   return check_launch("nvfp4_dyn_multi_kernel");
+}
+
+int b200q_collect_fake_quant_nvfp4_multi(const void *descs, int n_desc, size_t total_ctas, int dtype, float *slots,
+                                         const void *amax_base, int amax_dtype, b200q_stream_t stream) {
+  if (n_desc == 0 || total_ctas == 0) return B200Q_OK;
+  B200Q_REQUIRE(descs != nullptr && slots != nullptr && amax_base != nullptr && n_desc > 0, "null pointer");
+  B200Q_REQUIRE(dtype_ok(amax_dtype), "unknown amax dtype %d", amax_dtype);
+  B200Q_REQUIRE(total_ctas <= 0x7fffffffu, "too many CTAs");
+  const MultiDesc *d = static_cast<const MultiDesc *>(descs);
+  uint32_t *sl = reinterpret_cast<uint32_t *>(slots);
+  B200Q_DISPATCH_DTYPE(dtype, Tag,
+                       launch_pdl(nvfp4_dyn_multi_kernel<Tag, 32, 2, true>, dim3((unsigned)total_ctas), dim3(kNvThreads),
+                                  0, (cudaStream_t)stream, d, n_desc, amax_base, amax_dtype, sl));
+  return check_launch("nvfp4_dyn_multi_kernel<collect>");
+}
+
+int b200q_fake_quant_nvfp4_multi_fixup(const void *descs, const void *live, int n_desc, int dtype,
+                                       const float *slots, const void *amax_base, int amax_dtype, int *redo_count,
+                                       b200q_stream_t stream) {
+  if (n_desc == 0) return B200Q_OK;
+  B200Q_REQUIRE(descs != nullptr && live != nullptr && slots != nullptr && amax_base != nullptr &&
+                    redo_count != nullptr && n_desc > 0,
+                "null pointer");
+  B200Q_REQUIRE(dtype_ok(amax_dtype), "unknown amax dtype %d", amax_dtype);
+  const MultiDesc *d = static_cast<const MultiDesc *>(descs);
+  const unsigned long long *lf = static_cast<const unsigned long long *>(live);
+  const uint32_t *sl = reinterpret_cast<const uint32_t *>(slots);
+  B200Q_DISPATCH_DTYPE(dtype, Tag,
+                       return launch_nvfp4_fixup<Tag>(d, lf, n_desc, sl, amax_base, amax_dtype, redo_count,
+                                                      (cudaStream_t)stream));
+  return B200Q_OK;
 }
 
 int b200q_fake_quant_nvfp4_static(const void *x, void *y, int dtype, size_t n_blocks,

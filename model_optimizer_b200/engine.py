@@ -107,6 +107,10 @@ class ShardedPTQEngine:
         # grouped = ONE multi-tensor launch for the collect of all owned quantizers and ONE for their NVFP4 fake
         # quant (pointer-array kernels) instead of one launch per quantizer
         self.grouped = bool(grouped) and qformat == "nvfp4"
+        # grouped graph steps: number of quantizers whose fake quant the fix-up redid since reset() (int32 device
+        # scalar); in a steady state, where no batch sets a new running max, it stops growing
+        self.redo_count = torch.zeros(1, dtype=torch.int32, device=self.device) if self.grouped else None
+        self._fixup_bytes = 0
         self._step = 0
         self.comm_log = {"allreduce_calls": 0, "p2p_calls": 0, "p2p_bytes": 0}
         # layer sharding: a rank's fake quant only needs the amax of its OWN layers, which is complete
@@ -204,33 +208,47 @@ class ShardedPTQEngine:
         for (_, q, _), x in zip(self.quantizers, acts):
             q._calibrator.collect(x)
 
-    def _tables(self, acts, outs, parity):
-        """Descriptor tables of a parity's static buffers: every owned quantizer's activation with its arena slot,
-        and the same with its fake-quant destination (a ring of ``outs``; the hand-off buffer for the last o_proj)."""
+    def _table(self, acts, outs, parity):
+        """Descriptor table of a parity's static buffers for the fused collect + fake quant: every owned quantizer's
+        activation with its arena slot and its fake-quant destination (a ring of ``outs``; the hand-off buffer for the
+        last o_proj).  Raises if an output overlaps an activation or two outputs overlap other than as prefixes of one
+        buffer."""
         idx = {n: i for i, n in enumerate(self.arena.names())}
         slots = [idx[qn] for qn, _, _ in self.quantizers]
         n = len(outs)
         last_hidden = len(self.quantizers) - 4 if (self.handoff and self.hand_out is not None) else -1
         ys = [self.hand_out[parity] if i == last_hidden else outs[i % n][: x.numel()].view_as(x)
               for i, x in enumerate(acts)]
-        return (ops.TensorTable(acts, slots, None, "vec32"), ops.TensorTable(acts, slots, ys, "block16"))
+        return ops.TensorTable(acts, slots, ys, "block16", fused=True)
 
     def _capture_set(self, acts, outs, parity, side):
         g_collect, g_export, g_fq = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
         if self.grouped:
-            t_collect, t_fq = self._tables(acts, outs, parity)
+            # ONE read of every activation per step: the fused pass fake-quantizes with the amax exported by the
+            # previous step while it collects; the fix-up redoes the (rare) entries whose exported amax changes.
+            # Graph keys: "fake_quant" is the fused pass (the NVFP4 grid, 4 B per element), "collect" the fix-up.
+            t = self._table(acts, outs, parity)
+            self._fixup_bytes = t.fixup_bytes
+            arena = self.arena.freeze()
+
+            def fused():
+                ops.collect_fake_quant_nvfp4_multi(t, arena, self.amax_arena)
+
+            def fixup():
+                ops.fake_quant_nvfp4_multi_fixup(t, arena, self.amax_arena, self.redo_count)
+
             with torch.cuda.stream(side):
-                ops.amax_per_tensor_multi_(self.arena.freeze(), t_collect)
-                ops.fake_quant_nvfp4_multi(t_fq, self.amax_arena)
+                fused()
+                fixup()
             torch.cuda.synchronize(self.device)
             self.reset()
+            with torch.cuda.graph(g_fq, stream=side):
+                fused()
             with torch.cuda.graph(g_collect, stream=side):
-                ops.amax_per_tensor_multi_(self.arena.freeze(), t_collect)
+                fixup()
             with torch.cuda.graph(g_export, stream=side):
                 self.export_amax()
-            with torch.cuda.graph(g_fq, stream=side):
-                ops.fake_quant_nvfp4_multi(t_fq, self.amax_arena)
-            return {"collect": g_collect, "export": g_export, "fake_quant": g_fq, "tables": (t_collect, t_fq)}
+            return {"collect": g_collect, "export": g_export, "fake_quant": g_fq, "tables": (t,)}
         with torch.cuda.graph(g_collect, stream=side):
             self.collect(acts)
         with torch.cuda.graph(g_export, stream=side):
@@ -269,6 +287,8 @@ class ShardedPTQEngine:
     def reset(self):
         self.arena.freeze().zero_()
         self.amax_arena.zero_()
+        if self.redo_count is not None:
+            self.redo_count.zero_()
 
     # ---- CUDA graphs -----------------------------------------------------------------------------------
     def capture(self, acts, outs):
@@ -340,7 +360,8 @@ class ShardedPTQEngine:
         self.comm_log["p2p_bytes"] += sum(r.tensor.numel() * r.tensor.element_size() for r in reqs)
 
     def step_graph(self):
-        """One batch: collect -> export -> fake quant as graph replays.  Communication stream, overlapped: the
+        """One batch as graph replays: collect -> export -> fake quant, or with ``grouped`` the fused collect + fake
+        quant -> fix-up -> export (same results).  Communication stream, overlapped: the
         hidden-state hand-off of the PREVIOUS step's output (every step) and the arena all-reduce (once per
         ``allreduce_every`` batches)."""
         p = self._step & 1 if self.handoff else 0
@@ -352,9 +373,14 @@ class ShardedPTQEngine:
                 # the exchange issued one step ago (parity p) delivered this step's input and released hand_out[p]
                 main.wait_event(self._ev_comm[p])
             self._exchange(1 - p)                         # previous step's output travels under this step's kernels
-        g["collect"].replay()
-        g["export"].replay()
-        g["fake_quant"].replay()
+        if self.grouped:
+            g["fake_quant"].replay()
+            g["collect"].replay()
+            g["export"].replay()
+        else:
+            g["collect"].replay()
+            g["export"].replay()
+            g["fake_quant"].replay()
         if self.handoff:
             self._ev_step_done[p].record(main)
         self._step += 1
@@ -375,10 +401,12 @@ class ShardedPTQEngine:
         return 3 if self.grouped else 2 * len(self.quantizers) + 1
 
     def act_bytes_per_step(self) -> tuple[int, int]:
-        """(collect bytes, fake-quant bytes) of algorithmic HBM traffic for one batch on this rank."""
+        """(collect bytes, fake-quant bytes) of algorithmic HBM traffic for one batch on this rank.  ``grouped``: the
+        collect rides on the fake-quant read, and the first item is the fix-up's traffic when no exported amax changes
+        (the contested output ranges it rewrites, ``ops.live_block_ranges``; known once captured)."""
         elems = sum(self.tokens * cin for _, _, cin in self.quantizers)
         es = torch.empty((), dtype=self.dtype).element_size()
-        return elems * es, 2 * elems * es
+        return self._fixup_bytes if self.grouped else elems * es, 2 * elems * es
 
     # ---- weights -----------------------------------------------------------------------------------------
     def weight_pass(self, weights):

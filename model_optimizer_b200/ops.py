@@ -7,6 +7,7 @@ CPU tensors raise -- there is no fallback path.
 
 from __future__ import annotations
 
+import bisect
 import functools
 
 import torch
@@ -107,15 +108,62 @@ def histogram_(hist: torch.Tensor, x: torch.Tensor, range_max: torch.Tensor, tak
     return hist
 
 
+def live_block_ranges(inputs, outputs, block_bytes: int) -> list[tuple[int, int]]:
+    """For a table whose entries run in order, entry i reading ``inputs[i]`` and writing ``outputs[i]`` (both
+    ``(address, nbytes)``), per entry ``(live_from, contested_to)`` in ``block_bytes`` blocks of its output:
+    ``live_from`` is the first block that no LATER entry writes, so blocks ``[live_from, n)`` are the ones the entry
+    leaves in the buffer and the live ranges of all entries are disjoint; ``[live_from, contested_to)`` is the part of
+    that range an EARLIER entry writes too.  One grid over the table runs the entries concurrently, so that part may end
+    up holding the earlier entry's result; rewriting it afterwards (and all of ``[live_from, n)`` for an entry whose
+    result changed) leaves every output buffer as running the entries in order leaves it.  Raises
+    :class:`B200QuantError` when an output overlaps any input, or two outputs overlap without starting at the same
+    address (a later output must cover a prefix of an earlier one)."""
+    if len(inputs) != len(outputs):
+        raise B200QuantError("one output per input")
+    spans = sorted((a, a + n) for a, n in inputs if n > 0)
+    starts = [s for s, _ in spans]
+    reach, r = [], 0                                   # reach[k]: largest end among the first k + 1 inputs by start
+    for _, e in spans:
+        r = max(r, e)
+        reach.append(r)
+    for a, n in outputs:
+        k = bisect.bisect_left(starts, a + n)          # inputs starting below the output's end
+        if n > 0 and k > 0 and reach[k - 1] > a:
+            raise B200QuantError("fused collect + fake quant: an output overlaps an input")
+    ends = {}                                          # output base address -> largest extent
+    for a, n in outputs:
+        if n > 0:
+            ends[a] = max(ends.get(a, a), a + n)
+    r = 0
+    for a in sorted(ends):
+        if a < r:
+            raise B200QuantError("fused collect + fake quant: outputs overlap without sharing a base address")
+        r = max(r, ends[a])
+    live, after = [0] * len(outputs), {}               # after[base]: blocks written by the entries after i
+    for i in range(len(outputs) - 1, -1, -1):
+        a, n = outputs[i]
+        live[i] = min(n // block_bytes, after.get(a, 0))
+        after[a] = max(after.get(a, 0), n // block_bytes)
+    ranges, before = [], {}                            # before[base]: blocks written by the entries before i
+    for i, (a, n) in enumerate(outputs):
+        ranges.append((live[i], max(live[i], min(n // block_bytes, before.get(a, 0)))))
+        before[a] = max(before.get(a, 0), n // block_bytes)
+    return ranges
+
+
 class TensorTable:
     """Device descriptor table for the multi-tensor launches (``b200q_amax_per_tensor_multi`` /
     ``b200q_fake_quant_nvfp4_multi``): build once per set of (static) buffers, launch many times -- e.g. inside a
     CUDA graph.  ``xs`` (and ``ys``): contiguous CUDA tensors of one dtype, 32-byte aligned; ``slots``: the amax slot
-    index of each tensor."""
+    index of each tensor.  ``fused`` (NVFP4 with ``ys``): a table for ``collect_fake_quant_nvfp4_multi`` /
+    ``fake_quant_nvfp4_multi_fixup``, which also ships each entry's live output range (``live_block_ranges``) and
+    refuses buffers those launches cannot reproduce the sequential result on."""
 
-    def __init__(self, xs, slots=None, ys=None, unit: str = "vec32"):
+    def __init__(self, xs, slots=None, ys=None, unit: str = "vec32", fused: bool = False):
         if not xs:
             raise B200QuantError("empty tensor list")
+        if fused and (ys is None or unit != "block16"):
+            raise B200QuantError("a fused table needs outputs and unit='block16'")
         self.dtype = xs[0].dtype
         self.device = xs[0].device
         es = xs[0].element_size()
@@ -141,6 +189,14 @@ class TensorTable:
         self.total_ctas = first
         self.n = len(rows)
         self.table = torch.tensor(rows, dtype=torch.int64).to(self.device)
+        self.live = None
+        if fused:
+            nb = [x.numel() * es for x in xs]
+            live = live_block_ranges([(x.data_ptr(), n) for x, n in zip(xs, nb)],
+                                     [(y.data_ptr(), n) for y, n in zip(ys, nb)], 16 * es)
+            self.live = torch.tensor(live, dtype=torch.int64).to(self.device)
+            # bytes the fix-up moves when no amax changes: the contested ranges are read and written again
+            self.fixup_bytes = sum(c - f for f, c in live) * 16 * es * 2
         self._keep = (list(xs), None if ys is None else list(ys))  # the table holds raw pointers
 
 
@@ -160,6 +216,40 @@ def fake_quant_nvfp4_multi(table: TensorTable, amax_base: torch.Tensor):
     with torch.cuda.device(table.device):
         call("b200q_fake_quant_nvfp4_multi", table.table.data_ptr(), table.n, table.total_ctas, _DT[table.dtype],
              amax_base.data_ptr(), _DT[amax_base.dtype], torch.cuda.current_stream(table.device).cuda_stream)
+
+
+def _fused_args(table: TensorTable, slots: torch.Tensor, amax_base: torch.Tensor):
+    if table.live is None:
+        raise B200QuantError("the table was not built with fused=True")
+    _slots(slots)
+    if not amax_base.is_cuda or not amax_base.is_contiguous() or amax_base.dtype not in _DT:
+        raise B200QuantError("amax_base must be a contiguous CUDA tensor (fp32 / fp16 / bf16)")
+
+
+def collect_fake_quant_nvfp4_multi(table: TensorTable, slots: torch.Tensor, amax_base: torch.Tensor):
+    """``fake_quant_nvfp4_multi(table, amax_base)`` and ``amax_per_tensor_multi_(slots, table)`` in ONE read of every
+    input: the outputs are SPECULATIVE (quantized with the amax ``amax_base`` holds now, i.e. the previous export) until
+    ``fake_quant_nvfp4_multi_fixup`` has run.  ``table``: built with ``fused=True``."""
+    _fused_args(table, slots, amax_base)
+    with torch.cuda.device(table.device):
+        call("b200q_collect_fake_quant_nvfp4_multi", table.table.data_ptr(), table.n, table.total_ctas,
+             _DT[table.dtype], slots.data_ptr(), amax_base.data_ptr(), _DT[amax_base.dtype],
+             torch.cuda.current_stream(table.device).cuda_stream)
+
+
+def fake_quant_nvfp4_multi_fixup(table: TensorTable, slots: torch.Tensor, amax_base: torch.Tensor,
+                                 redo_count: torch.Tensor):
+    """Between ``collect_fake_quant_nvfp4_multi`` and the export of ``slots`` into ``amax_base``: redo, with the new
+    amax, the entries whose exported amax is about to change, and rewrite the contested part of every live output range
+    (``live_block_ranges``), so that after the export everything is bit-identical to collect -> export -> fake quant.
+    ``redo_count`` (int32 CUDA scalar) += number of entries redone."""
+    _fused_args(table, slots, amax_base)
+    if redo_count.dtype != torch.int32 or not redo_count.is_cuda or redo_count.numel() != 1:
+        raise B200QuantError("redo_count must be an int32 CUDA tensor of one element")
+    with torch.cuda.device(table.device):
+        call("b200q_fake_quant_nvfp4_multi_fixup", table.table.data_ptr(), table.live.data_ptr(), table.n,
+             _DT[table.dtype], slots.data_ptr(), amax_base.data_ptr(), _DT[amax_base.dtype], redo_count.data_ptr(),
+             torch.cuda.current_stream(table.device).cuda_stream)
 
 
 def hist_plan_(plan_state: torch.Tensor, batch_amax: torch.Tensor, nbins0: int, capacity: int) -> torch.Tensor:

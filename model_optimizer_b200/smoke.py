@@ -62,6 +62,15 @@ def run():
     ys = [torch.empty_like(t) for t in xs]
     ops.fake_quant_nvfp4_multi(ops.TensorTable(xs, None, ys, "block16"), slots)
     assert torch.equal(ys[0], ops.fake_quant_nvfp4(x, slot))
+    # fused collect + fake quant from reset (speculative amax 0: both entries are redone) + fix-up + export
+    slots2, amax2 = torch.zeros_like(slots), torch.zeros_like(slots)
+    ys2, redo = [torch.empty_like(t) for t in xs], torch.zeros(1, dtype=torch.int32, device="cuda")
+    t_fused = ops.TensorTable(xs, None, ys2, "block16", fused=True)
+    ops.collect_fake_quant_nvfp4_multi(t_fused, slots2, amax2)
+    ops.fake_quant_nvfp4_multi_fixup(t_fused, slots2, amax2, redo)
+    amax2.copy_(slots2)
+    assert torch.equal(slots2, slots) and int(redo) == 2, "fused collect mismatch"
+    assert all(torch.equal(a, b) for a, b in zip(ys2, ys)), "fused fake quant mismatch"
     from .calib import HistogramCalibrator
 
     hc = HistogramCalibrator(8, None, False, num_bins=512)
@@ -81,5 +90,5 @@ def run():
     ref_l = o.mse_sweep_losses_rows(xh, a0, mult.cpu().numpy(), 8, False, False, "bf16", round_mult=True)
     assert np.allclose(loss.cpu().numpy(), ref_l, rtol=1e-5), "per-row MSE sweep mismatch"
     torch.cuda.synchronize()
-    print("smoke ok: collect / fake quant (NVFP4, FP8, INT8) / pack (NVFP4, INT4) / grouped launches / histogram + "
+    print("smoke ok: collect / fake quant (NVFP4, FP8, INT8) / pack (NVFP4, INT4) / grouped and fused launches / histogram + "
           "amax searches / MSE sweep match the oracle")
