@@ -392,6 +392,26 @@ int b200q_nvfp4_fp8_scale_sweep_hessian(const void *w, int dtype, size_t cout, s
                                         const float *cand_scales, const float *cand_amaxes, int n_cand,
                                         const float *hessian, float *best_amax, b200q_stream_t stream);
 
+/* ---- (4) input rotation (normalized Hadamard transform) --------------------------------- */
+
+/* Normalized fast Walsh-Hadamard transform over contiguous blocks of block_size = 2^k elements (k = 0..15) along
+ * the last dim of x [n_rows, row_len] (row_len % block_size == 0).  Per block: widen to fp32; stages s = 0..k-1 in
+ * ascending order, each mapping the pair (i, i | 2^s) with bit s of i clear to (a + b, a - b) with separate fp32
+ * round-to-nearest adds; one multiply by fl32(block_size^-0.5); one RNE rounding to dtype.  y must not alias x.
+ * amax_slot (may be null): amax_slot[0] = max(amax_slot[0], max |y|) over the rounded outputs, with the rule of
+ * b200q_amax_per_tensor (NaN propagates) -- the collect of a per-tensor max calibrator of the rotated input.
+ * Replaces fast_hadamard_transform.hadamard_transform(x.reshape(-1, row_len / block_size, block_size),
+ * scale=block_size ** -0.5) as called by normalized_hadamard_transform (quantization/nn/functional.py:81-138). */
+int b200q_hadamard(const void *x, void *y, int dtype, size_t n_rows, size_t row_len, size_t block_size,
+                   float *amax_slot, b200q_stream_t stream);
+/* y = fake_quant_nvfp4(hadamard(x)) (rotate_back = 0) or hadamard(fake_quant_nvfp4(hadamard(x))) (rotate_back = 1)
+ * in one pass, bit-identical to those calls of b200q_hadamard and b200q_fake_quant_nvfp4: the rotated NVFP4
+ * quantizer of TensorQuantizer.forward (quantization/nn/modules/tensor_quantizer.py:1146-1219).
+ * row_len % 16 == 0 and row_len % block_size == 0; global_amax as in b200q_fake_quant_nvfp4. */
+int b200q_fake_quant_nvfp4_rotated(const void *x, void *y, int dtype, size_t n_rows, size_t row_len,
+                                   size_t block_size, int rotate_back, const void *global_amax, int amax_dtype,
+                                   b200q_stream_t stream);
+
 /* ---- self tests (device-side numerics used by tests/, not by the product path) ----------- */
 /* Checks the hoisted-reciprocal exact division against div.rn.f32 on n pseudo-random pairs
  * (seeded); returns the number of mismatches in *mismatches_host. */

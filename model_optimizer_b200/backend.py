@@ -1,5 +1,5 @@
 """Drop-in installation into a real ``modelopt`` (when it is importable): the sanctioned hooks of
-SURVEY.md 8(b), plus the three module-level functions the hooks cannot reach.
+SURVEY.md 8(b), plus the module-level functions the hooks cannot reach.
 
 1. ``register_quant_backend("b200", entrypoint)`` (nn/modules/tensor_quantizer.py:87-109): fake quant of
    any quantizer whose config carries ``backend: "b200"`` runs the fused sm_90a kernels.
@@ -19,7 +19,10 @@ SURVEY.md 8(b), plus the three module-level functions the hooks cannot reach.
    * ``NVFP4QTensor.quantize`` / ``FP8QTensor.quantize`` (qtensor/nvfp4_tensor.py:253, qtensor/fp8_tensor.py:41):
      the weight quant-and-pack of ``mtq.compress`` / ``TensorQuantizer._real_quantize`` (:796-887) is pure ATen
      in the reference; here one pack kernel each.  Calls outside the engine's scope (CPU tensors,
-     pre-computed block scales, ``keep_high_precision``) are handed back to the host application's own function.
+     pre-computed block scales, ``keep_high_precision``) are handed back to the host application's own function;
+   * ``normalized_hadamard_transform`` as named in ``nn/modules/tensor_quantizer.py`` (:67, called by
+     ``_rotate_inputs`` :664-668): every ``rotate`` config on CUDA tensors runs ``b200q_hadamard`` instead of needing
+     the external ``fast_hadamard_transform`` package (other inputs go to the host application's own function).
 
 Nothing here is imported by the engine itself; ``install()`` raises if modelopt is absent.
 ``stats`` counts kernel-path calls per hook so a test can prove which side executed.
@@ -34,6 +37,7 @@ import types
 import torch
 
 from . import ops
+from .nn.functional import normalized_hadamard_transform
 from .tensor_quant import dynamic_block_quant, fake_tensor_quant, scaled_e4m3, static_blockwise_fp4_fake_quant
 
 stats: collections.Counter = collections.Counter()
@@ -330,11 +334,21 @@ def install(patch_extensions: bool = True, patch_functions: bool = True):
             return mine(x, amax, global_amax, quantize_block_scales, fp8_max_for_normalization, out_dtype,
                         pass_through_bwd)
 
+        orig_hadamard = ref_tq.normalized_hadamard_transform
+
+        def hadamard(inputs, rotate_fp32=False, block_size=None):
+            if not inputs.is_cuda or inputs.dtype not in ops._DT:      # outside the engine: the host's own function
+                return orig_hadamard(inputs, rotate_fp32=rotate_fp32, block_size=block_size)
+            stats["fn.normalized_hadamard_transform"] += 1
+            return normalized_hadamard_transform(inputs, rotate_fp32, block_size)
+
         _saved["fn"] = {"static": ref_tq.static_blockwise_fp4_fake_quant,
                         "nvfp4_quantize": NVFP4QTensor.__dict__["quantize"],
                         "fp8_quantize": FP8QTensor.__dict__["quantize"],
-                        "mse": ref_model_calib.MseCalibrator}
+                        "mse": ref_model_calib.MseCalibrator,
+                        "hadamard": orig_hadamard}
         ref_tq.static_blockwise_fp4_fake_quant = static_fp4
+        ref_tq.normalized_hadamard_transform = hadamard
         ref_model_calib.MseCalibrator = _make_mse_factory(base, ref_model_calib.MseCalibrator)
         NVFP4QTensor.quantize, FP8QTensor.quantize = _make_qtensor_patches(NVFP4QTensor, FP8QTensor)
     return B200MaxCalibrator, B200HistogramCalibrator
@@ -353,6 +367,7 @@ def uninstall():
         import modelopt.torch.quantization.model_calib as ref_model_calib
 
         ref_tq.static_blockwise_fp4_fake_quant = fn["static"]
+        ref_tq.normalized_hadamard_transform = fn["hadamard"]
         ref_model_calib.MseCalibrator = fn["mse"]
         NVFP4QTensor.quantize = fn["nvfp4_quantize"]
         FP8QTensor.quantize = fn["fp8_quantize"]

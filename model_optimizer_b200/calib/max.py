@@ -88,6 +88,18 @@ class MaxCalibrator(_Calibrator):
         if self._track_amax:
             self._amaxs.append(self._slots.clone().reshape(shape).cpu().numpy())
 
+    def tensor_slot(self, x: torch.Tensor) -> torch.Tensor:
+        """The fp32 slot of a per-tensor calibrator (created for x on first use), for a kernel that folds its own |y|
+        max into it in place of ``collect`` (``ops.hadamard``)."""
+        if self._axis is not None or self._track_amax:
+            raise RuntimeError("tensor_slot: per-tensor calibrators without amax tracking only")
+        if self._slots is None:
+            self._slots = torch.zeros(1, dtype=torch.float32, device=x.device)
+            self._shape, self._dtype = (), x.dtype
+        elif self._slots.numel() != 1 or self._shape != ():
+            raise RuntimeError("amax shape changed!")
+        return self._slots
+
     def reset(self):
         self._slots = None
         self._shape = None

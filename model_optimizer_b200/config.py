@@ -2,7 +2,7 @@
 
 Mirrors the part of ``modelopt/torch/quantization/config.py`` the hot path reads
 (``QuantizerAttributeConfig`` :322-709 -- ``num_bits, axis, block_sizes, fake_quant, unsigned,
-narrow_range, calibrator, enable``) and the preset dictionaries (:1681-1778), which are ordered
+narrow_range, calibrator, enable, rotate``) and the preset dictionaries (:1681-1778), which are ordered
 lists of ``{"quantizer_name": fnmatch pattern, "cfg": {...} | "enable": bool}`` entries plus an
 ``"algorithm"``.
 """
@@ -10,8 +10,31 @@ lists of ``{"quantizer_name": fnmatch pattern, "cfg": {...} | "enable": bool}`` 
 from __future__ import annotations
 
 import copy
+import dataclasses
 from dataclasses import dataclass, field
 from typing import Any
+
+
+@dataclass
+class RotateConfig:
+    """quantization/config.py:282-319: normalized Hadamard rotation of the quantizer input (RHT / QuaRot / SpinQuant).
+    ``mode="rotate_back"`` applies the transform again after fake quantization; ``block_size`` None rotates the whole
+    last dim (or its largest power-of-2 divisor, nn/functional.py)."""
+
+    enable: bool = False
+    mode: str = "rotate"
+    rotate_fp32: bool = False
+    block_size: int | None = None
+
+    def __post_init__(self):
+        if self.mode not in ("rotate", "rotate_back"):
+            raise ValueError(f"rotate mode must be 'rotate' or 'rotate_back', got {self.mode!r}")
+        v = self.block_size
+        if v is not None and (isinstance(v, bool) or not isinstance(v, int) or v <= 0):
+            raise ValueError(f"block_size must be a positive int, got {v!r}")
+
+    def model_copy(self, update=None):
+        return dataclasses.replace(self, **(update or {}))
 
 
 @dataclass
@@ -33,6 +56,8 @@ class QuantizerAttributeConfig:
     bias: dict | None = None
     effective_bits: float | None = None  # informational (NVFP4 presets carry it)
     trt_high_precision_dtype: str = "Float"
+    # input rotation (config.py:616-625): a bool is RotateConfig(enable=...), a dict the RotateConfig fields
+    rotate: bool | dict | RotateConfig = False
 
     def __post_init__(self):
         if isinstance(self.num_bits, list):
@@ -52,6 +77,10 @@ class QuantizerAttributeConfig:
             assert any(isinstance(k, int) for k in self.bias), "The axis for bias computation is not specified."
         if self.type not in ("static", "dynamic"):
             raise ValueError(f"type must be 'static' or 'dynamic', got {self.type}")
+        if isinstance(self.rotate, dict):
+            self.rotate = RotateConfig(**self.rotate)
+        elif not isinstance(self.rotate, (bool, RotateConfig)):
+            raise ValueError(f"rotate must be a bool, a dict or a RotateConfig, got {self.rotate!r}")
 
 
 _DEFAULT_DISABLED = [
@@ -139,4 +168,4 @@ def get_preset(name: str) -> dict:
     return copy.deepcopy(PRESETS[name])
 
 
-__all__ = ["QuantizerAttributeConfig", "PRESETS", "get_preset", *PRESETS.keys()]
+__all__ = ["QuantizerAttributeConfig", "RotateConfig", "PRESETS", "get_preset", *PRESETS.keys()]

@@ -49,7 +49,8 @@ def _records(x, create: bool):
 def signature(q) -> tuple:
     bs = q._block_sizes
     return (str(q._num_bits), str(q._axis), None if bs is None else tuple(sorted((str(k), str(v)) for k, v in bs.items())),
-            q._unsigned, q._narrow_range, q._dynamic, q._fake_quant, type(q._calibrator).__name__)
+            q._unsigned, q._narrow_range, q._dynamic, q._fake_quant, type(q._calibrator).__name__,
+            (q.rotate_is_enabled, q.rotate_back_is_enabled, q.rotate_block_size))
 
 
 def eligible(q, x) -> bool:

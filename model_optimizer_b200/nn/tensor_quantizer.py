@@ -1,7 +1,7 @@
 """TensorQuantizer -- host-side mirror of
 ``modelopt/torch/quantization/nn/modules/tensor_quantizer.py`` (``TensorQuantizer`` :136,
 ``forward`` :1119-1221, ``_fake_quantize`` :890-949, ``_get_amax`` :736-751, ``collect`` :1397-1407,
-static block reshape :975-1061, ``load_calib_amax`` :697-720, ``export_amax`` :1082-1117).
+static block reshape :975-1061, ``load_calib_amax`` :697-720, ``export_amax`` :1082-1117, input rotation :616-668).
 
 Same attribute names and state (``_amax`` buffer in the input dtype, ``_pre_quant_scale``,
 ``_if_quant`` / ``_if_calib`` / ``_disabled``), same dispatch rules; every numeric step is a
@@ -17,8 +17,9 @@ import torch.nn.functional as F
 from torch import nn
 
 from .. import calib, ops
-from ..config import QuantizerAttributeConfig
+from ..config import QuantizerAttributeConfig, RotateConfig
 from . import shared_input as _shared
+from .functional import normalized_hadamard_transform, rotate_block_size
 from ..tensor_quant import dynamic_block_quant, fake_tensor_quant, scaled_e4m3, static_blockwise_fp4_fake_quant
 
 
@@ -73,6 +74,7 @@ class TensorQuantizer(nn.Module):
         self._disabled = not cfg.enable
         self._dynamic = cfg.type == "dynamic"
         self._bias = dict(cfg.bias) if cfg.bias else None
+        self._rotate = cfg.rotate
         self._bias_calibrator = None
         if hasattr(self, "_bias_value"):
             delattr(self, "_bias_value")
@@ -259,6 +261,77 @@ class TensorQuantizer(nn.Module):
             self.register_buffer("_pre_quant_scale", value.clone().detach())
         else:
             self._pre_quant_scale.data.copy_(value.clone().detach().to(self._pre_quant_scale.device))
+
+    # ---- input rotation (tensor_quantizer.py:616-668) -------------------------------------------------
+    @property
+    def rotate_is_enabled(self):
+        if isinstance(self._rotate, RotateConfig):
+            return self._rotate.enable
+        if isinstance(self._rotate, dict):  # a state dict of an older checkpoint
+            return self._rotate.get("enable", False)
+        return self._rotate
+
+    @property
+    def rotate_is_fp32(self):
+        if isinstance(self._rotate, RotateConfig):
+            return self._rotate.rotate_fp32 if self._rotate.enable else False
+        if isinstance(self._rotate, dict) and self.rotate_is_enabled:
+            return self._rotate.get("rotate_fp32", False)
+        return False
+
+    @property
+    def rotate_block_size(self):
+        if isinstance(self._rotate, RotateConfig):
+            return self._rotate.block_size if self._rotate.enable else None
+        if isinstance(self._rotate, dict) and self.rotate_is_enabled:
+            return self._rotate.get("block_size", None)
+        return None
+
+    @property
+    def rotate_back_is_enabled(self):
+        if isinstance(self._rotate, RotateConfig):
+            return self._rotate.enable and self._rotate.mode == "rotate_back"
+        if isinstance(self._rotate, dict) and self.rotate_is_enabled:
+            return self._rotate.get("mode", "rotate") == "rotate_back"
+        return False
+
+    def disable_rotate(self):
+        """Disable rotation, keeping the type of the ``_rotate`` field (idempotent)."""
+        self._state_gen += 1
+        if isinstance(self._rotate, RotateConfig):
+            self._rotate = self._rotate.model_copy(update={"enable": False})
+        elif isinstance(self._rotate, dict):
+            self._rotate = dict(self._rotate, enable=False)
+        else:
+            self._rotate = False
+
+    def _rotate_inputs(self, inputs, amax_slot=None):
+        if amax_slot is not None:  # the collect of a per-tensor max calibrator, folded into the transform
+            return normalized_hadamard_transform(inputs, rotate_fp32=self.rotate_is_fp32,
+                                                 block_size=self.rotate_block_size, amax_slot=amax_slot)
+        return normalized_hadamard_transform(inputs, rotate_fp32=self.rotate_is_fp32, block_size=self.rotate_block_size)
+
+    def _rotate_collect_slot(self, inputs):
+        """The fp32 slot the transform can fold the calibration collect into (per-tensor ``MaxCalibrator``, no bias,
+        no block reshape or axis conversion before the collect), or None."""
+        cal = self._calibrator
+        if not (self._if_calib and not self._dynamic and isinstance(cal, calib.MaxCalibrator) and cal._axis is None
+                and not cal._track_amax and self._bias is None and inputs.is_cuda
+                and (self._block_sizes is None or self.is_nvfp4_dynamic)):
+            return None
+        return cal.tensor_slot(inputs)
+
+    def _fake_quant_rotated_nvfp4(self, inputs):
+        """NVFP4 dynamic block fake quant of the rotated input (rotated back for ``rotate_back``) in one kernel when the
+        quantizer has a calibrated per-tensor amax, is not calibrating and no autograd graph is needed; else None."""
+        amax = getattr(self, "_amax", None)
+        if not (self.is_nvfp4_dynamic and self._if_quant and self._fake_quant and not self._disabled
+                and not (self._if_calib and not self._dynamic) and amax is not None and amax.numel() == 1
+                and inputs.is_cuda and inputs.dim() > 0 and inputs.shape[-1] % 16 == 0
+                and not (torch.is_grad_enabled() and inputs.requires_grad)):
+            return None
+        bs = rotate_block_size(inputs.shape[-1], self.rotate_block_size)
+        return ops.fake_quant_nvfp4_rotated(inputs, bs, amax, self.rotate_back_is_enabled)
 
     # ---- mode switches (tensor_quantizer.py:640-695) ---------------------------------------------------
     def disable(self):
@@ -531,10 +604,25 @@ class TensorQuantizer(nn.Module):
                 inputs = ops.scale_cols(inputs, pqs.reshape(-1))
             else:
                 inputs = inputs * pqs
+        rotate, rotate_back = self.rotate_is_enabled, self.rotate_back_is_enabled
+        if rotate_back and self._if_quant and not self._fake_quant:   # tensor_quantizer.py:1146-1147, before rotating
+            raise ValueError("rotate_back mode is only supported with fake_quant=True.")
         if self._disabled or not (self._if_quant or (self._if_calib and not self._dynamic)):
             # nothing to do in this phase (e.g. a weight quantizer held during the activation calibration loop): the
-            # reference reshapes into blocks and back for the same values
+            # reference reshapes into blocks and back for the same values.  It still rotates (and rotates back)
+            if rotate:
+                inputs = self._rotate_inputs(inputs)
+                if rotate_back:
+                    inputs = self._rotate_inputs(inputs)
             return inputs
+        collected = False
+        if rotate:
+            fused = self._fake_quant_rotated_nvfp4(inputs)
+            if fused is not None:
+                return fused
+            slot = self._rotate_collect_slot(inputs)
+            inputs = self._rotate_inputs(inputs, slot)
+            collected = slot is not None
         if self._block_sizes is not None and self._fake_quant:
             self._block_sizes_to_axis(inputs)
         if self.is_static_block_quant:
@@ -545,13 +633,13 @@ class TensorQuantizer(nn.Module):
         if self._if_calib and not self._dynamic:
             if self._calibrator is None:
                 raise RuntimeError("Calibrator was not created.")
-            if not share or _shared.collect_once(self, inputs):
+            if not collected and (not share or _shared.collect_once(self, inputs)):
                 self.collect(inputs)
         if self._if_quant:
             if share and self._fake_quant:
                 hit = _shared.cached_output(self, inputs)
                 if hit is not None:
-                    return hit
+                    return self._rotate_inputs(hit) if rotate_back else hit
             src = inputs
             if not inputs.is_contiguous():
                 inputs = inputs.contiguous()
@@ -566,15 +654,26 @@ class TensorQuantizer(nn.Module):
                                  "This case should have been handled.")
         if self.is_static_block_quant and isinstance(outputs, torch.Tensor):
             outputs = self._reset_to_original_shape(outputs)
+        if rotate_back and isinstance(outputs, torch.Tensor):
+            outputs = self._rotate_inputs(outputs)
         return outputs
+
+    def _rotate_repr(self):
+        """tensor_quantizer.py:1250-1254."""
+        s = " rotated" if self.rotate_is_enabled else ""
+        s += " (rotate_back)" if self.rotate_back_is_enabled else ""
+        s += " (fp32)" if self.rotate_is_fp32 else ""
+        if self.rotate_block_size is not None:
+            s += f" (block={self.rotate_block_size})"
+        return s
 
     def extra_repr(self):
         if self._disabled:
-            return "disabled"
+            return "disabled" + self._rotate_repr()
         a = self.amax
         amax = "dynamic" if a is None else (f"{a.item():.4e}" if a.numel() == 1 else f"[{a.min().item():.2e}, {a.max().item():.2e}]({a.numel()})")
         return (f"{self._num_bits} bit fake={self._fake_quant} axis={self._axis} block_sizes={self._block_sizes} "
-                f"amax={amax} calib={self._if_calib} quant={self._if_quant}")
+                f"amax={amax} calib={self._if_calib} quant={self._if_quant}" + self._rotate_repr())
 
 
 __all__ = ["TensorQuantizer"]

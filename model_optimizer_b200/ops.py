@@ -393,6 +393,48 @@ def fake_quant_nvfp4(x, global_amax, out=None):
     return y
 
 
+HADAMARD_MAX_BLOCK = 32768
+
+
+def _hadamard_shape(x, block_size):
+    bs = int(block_size)
+    if bs < 1 or bs & (bs - 1) or bs > HADAMARD_MAX_BLOCK:
+        raise ValueError(f"Hadamard block_size must be a power of 2 no larger than {HADAMARD_MAX_BLOCK}, got {block_size}")
+    row_len = x.shape[-1] if x.dim() > 0 else 1
+    if row_len % bs:
+        raise ValueError(f"the last dim {row_len} is not a multiple of the Hadamard block_size {bs}")
+    return bs, row_len, (x.numel() // row_len if row_len else 0)
+
+
+def hadamard(x, block_size, amax_slot=None):
+    """Normalized Walsh-Hadamard transform of every contiguous block of ``block_size`` (a power of 2 up to 32768)
+    elements along the last dim: fp32 butterflies in ascending stage order, one multiply by fl32(block_size ** -0.5),
+    one rounding to x's dtype.  Returns a new tensor.  ``amax_slot`` (fp32 [1]): also folds max|y| into it, exactly as
+    ``amax_per_tensor_(amax_slot, y)`` would."""
+    bs, row_len, n_rows = _hadamard_shape(x, block_size)
+    x = _prep(x, "x")
+    if amax_slot is not None:
+        _slots(amax_slot, "amax_slot")
+    y = torch.empty_like(x)
+    call("b200q_hadamard", x.data_ptr(), y.data_ptr(), _dt(x), n_rows, row_len, bs,
+         None if amax_slot is None else amax_slot.data_ptr(), _stream(x))
+    return y
+
+
+def fake_quant_nvfp4_rotated(x, block_size, global_amax, rotate_back=False):
+    """``fake_quant_nvfp4(hadamard(x, block_size), global_amax)``, rotated back with ``hadamard`` when
+    ``rotate_back``: one pass, the same bits.  The last dim must be a multiple of 16 and of ``block_size``."""
+    bs, row_len, n_rows = _hadamard_shape(x, block_size)
+    x = _prep(x, "x")
+    if row_len % 16:
+        raise ValueError(f"rotated NVFP4 fake quant: the last dim {row_len} is not a multiple of 16")
+    global_amax = _amax_arg(global_amax, x)
+    y = torch.empty_like(x)
+    call("b200q_fake_quant_nvfp4_rotated", x.data_ptr(), y.data_ptr(), _dt(x), n_rows, row_len, bs, int(bool(rotate_back)),
+         global_amax.data_ptr(), _dt(global_amax), _stream(x))
+    return y
+
+
 def fake_quant_nvfp4_static(x, block_amax, global_amax=None, quantize_block_scales=True,
                             fp8_max_norm=448.0, out=None):
     """NVFP4 static fake quant: ``block_amax.numel() == x.numel() // 16`` calibrated amaxes."""

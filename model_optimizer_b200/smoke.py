@@ -89,6 +89,18 @@ def run():
     ops.mse_sweep_rows_(loss, x, torch.from_numpy(a0).cuda().to(torch.bfloat16).reshape(-1), mult, 8, False, False)
     ref_l = o.mse_sweep_losses_rows(xh, a0, mult.cpu().numpy(), 8, False, False, "bf16", round_mult=True)
     assert np.allclose(loss.cpu().numpy(), ref_l, rtol=1e-5), "per-row MSE sweep mismatch"
+    # (6) input rotation: the transform (with its folded collect), its round trip and the fused rotated NVFP4 pass
+    from tools.hadamard_oracle import hadamard as had_ref
+
+    rs = torch.zeros(1, dtype=torch.float32, device="cuda")
+    r = ops.hadamard(x, 128, rs)
+    assert np.array_equal(r.float().cpu().numpy().view(np.uint32), had_ref(xh, 128, "bf16").view(np.uint32)), \
+        "hadamard mismatch"
+    assert float(rs) == float(o.reduce_amax(r.float().cpu().numpy())), "rotated collect mismatch"
+    rr = ops.hadamard(r, 128)
+    assert float((rr.float() - x.float()).abs().max()) <= 2 ** -6 * float(x.float().abs().max()), "rotation round trip"
+    fused = ops.fake_quant_nvfp4_rotated(x, 128, rs.to(torch.bfloat16), True)
+    assert torch.equal(fused, ops.hadamard(ops.fake_quant_nvfp4(r, rs.to(torch.bfloat16)), 128)), "rotated NVFP4 mismatch"
     torch.cuda.synchronize()
     print("smoke ok: collect / fake quant (NVFP4, FP8, INT8) / pack (NVFP4, INT4) / grouped and fused launches / histogram + "
-          "amax searches / MSE sweep match the oracle")
+          "amax searches / MSE sweep / Hadamard rotation match the oracle")
