@@ -103,20 +103,25 @@ int b200q_fake_quant_nvfp4_multi(const void *descs, int n_desc, size_t total_cta
 
 /* One read of each activation for collect + fake quant, with a speculative amax and an exact fix-up:
  *   collect_fake_quant: b200q_fake_quant_nvfp4_multi (NVFP4 descs, amax = amax_base[slot], the value exported one step
- *                       earlier) that ALSO does b200q_amax_per_tensor_multi's slots[slot] = max(slots[slot], max|x|);
+ *                       earlier) that ALSO does b200q_amax_per_tensor_multi's slots[slot] = max(slots[slot], max|x|).
+ *                       Where outputs share a buffer, the caller launches it twice in stream order over sub-tensor
+ *                       descriptors: the second launch holds the tiles of 512 blocks that an entry writes last while
+ *                       an earlier entry writes them too (ops.second_pass_tiles), so their stores land last;
  *   fixup             : then, before the export, every entry whose slot rounded to amax_dtype as b200q_amax_export
  *                       rounds it differs in bits from amax_base[slot] is fake-quantized again with that new amax over
- *                       its live blocks [live[2i], n_units), every other entry over [live[2i], live[2i+1]) (live:
- *                       device array of n_desc x 2 uint64: the first block of entry i's output that no later entry
- *                       overwrites, and the end of the part of that range earlier entries write too);
- *                       *redo_count += number of entries whose amax changed.
+ *                       its live blocks [live[2i], n_units) (live: device array of n_desc x 2 uint64 from
+ *                       ops.live_block_ranges; live[2i] is the first block of entry i's output that no later entry
+ *                       overwrites), and the pieces (device array of n_pieces x 3 int64: entry, first block, end block)
+ *                       are fake-quantized again with the exported amax: the live blocks of the tiles where live
+ *                       blocks of two entries meet (ops.output_tiles).  *redo_count += number of entries whose amax
+ *                       changed.
  * After the export, outputs, slots and amax_base are bit-identical to collect -> export -> fake quant, provided no
  * output overlaps an input and outputs overlap only as prefixes of one buffer (same base pointer). */
 int b200q_collect_fake_quant_nvfp4_multi(const void *descs, int n_desc, size_t total_ctas, int dtype, float *slots,
                                          const void *amax_base, int amax_dtype, b200q_stream_t stream);
 int b200q_fake_quant_nvfp4_multi_fixup(const void *descs, const void *live, int n_desc, int dtype,
-                                       const float *slots, const void *amax_base, int amax_dtype, int *redo_count,
-                                       b200q_stream_t stream);
+                                       const float *slots, const void *amax_base, int amax_dtype, const void *pieces,
+                                       int n_pieces, int *redo_count, b200q_stream_t stream);
 
 /* amax search over a collected histogram (HistogramCalibrator.compute_amax, quantization/calib/histogram.py:137-343;
  * host-side NumPy / Python loops in the reference -- one CTA per candidate here).  hist: integer-valued fp32 counts.

@@ -39,7 +39,7 @@ _SIGNATURES = {
     "b200q_amax_per_tensor_multi": [_P, c_int, c_size_t, c_int, _P, _P],
     "b200q_fake_quant_nvfp4_multi": [_P, c_int, c_size_t, c_int, _P, c_int, _P],
     "b200q_collect_fake_quant_nvfp4_multi": [_P, c_int, c_size_t, c_int, _P, _P, c_int, _P],
-    "b200q_fake_quant_nvfp4_multi_fixup": [_P, _P, c_int, c_int, _P, _P, c_int, _P, _P],
+    "b200q_fake_quant_nvfp4_multi_fixup": [_P, _P, c_int, c_int, _P, _P, c_int, _P, c_int, _P, _P],
     "b200q_hist_search_percentile": [_P, c_int, ctypes.c_double, _P, _P],
     "b200q_hist_search_entropy": [_P, c_int, c_int, c_int, c_int, _P, _P, _P, _P],
     "b200q_hist_search_mse": [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P],

@@ -152,24 +152,60 @@ __global__ void __launch_bounds__(kNvThreads, !COLLECT ? 0 : std::is_same<Tag, B
   }
 }
 
-// Exact fix-up after a speculative COLLECT pass (which quantized with the amax exported one step earlier): an entry
-// whose new exported amax -- its fp32 slot rounded to amax_dtype as amax_export_kernel rounds it -- differs in bits
-// from amax_base[slot] (what the pass used; the export has not run yet) is quantized again with the new amax.
-// live[2 i], live[2 i + 1] = (live_from, contested_to) of entry i (ops.live_block_ranges).  Only its live blocks
-// [live_from, n_units) are redone: the prefix below live_from is overwritten by later entries of the table that share
-// the output buffer, and the live ranges of different entries never overlap.  An unchanged entry still rewrites
-// [live_from, contested_to), the part of its live range that earlier entries write too: the pass runs them
-// concurrently, so their stores may have landed after its own.  Each buffer then ends as the sequential launches leave
-// it.  Persistent grid: every CTA checks the entries 256 at a time (one per thread) and grid-strides over the range
-// of each one that has work; redo_count gets one increment per changed entry.
+// The amax the export is about to give entry e -- its fp32 slot rounded to amax_dtype as amax_export_kernel rounds
+// it -- and whether it differs in bits from amax_base[slot] (what the speculative pass used).
+__device__ __forceinline__ float exported_amax(const MultiDesc &d, const uint32_t *__restrict__ slots,
+                                               const void *__restrict__ amax_base, int amax_dtype, bool &changed) {
+  const long long slot = d.slot;
+  const float v = __uint_as_float(__ldcg(slots + slot));
+  uint32_t nb, ob;
+  float na;
+  if (amax_dtype == B200Q_F32) {
+    nb = __float_as_uint(v);
+    ob = static_cast<const uint32_t *>(amax_base)[slot];
+    na = v;
+  } else if (amax_dtype == B200Q_BF16) {
+    nb = f2bf_bits(v);
+    ob = static_cast<const uint16_t *>(amax_base)[slot];
+    na = __uint_as_float(nb << 16);
+  } else {
+    nb = f2h_bits(v);
+    ob = static_cast<const uint16_t *>(amax_base)[slot];
+    na = h2f_bits((uint16_t)nb);
+  }
+  changed = nb != ob;
+  return na;
+}
+
+// the whole CTA quantizes blocks [from, to) of entry d with amax a
+template <typename Tag, int VB, int UNROLL>
+__device__ __forceinline__ void cta_fq_range(const MultiDesc &d, size_t from, size_t to, float a) {
+  DynScale ds;
+  ds.setup(a);
+  const ExactDiv d6(ds.six_gs);
+  for (size_t i = from + threadIdx.x; i < to; i += (size_t)kNvThreads * UNROLL)
+    dyn_fq_blocks<Tag, VB, UNROLL, false>(d.x, d.y, i, kNvThreads, to, ds, d6);
+}
+
+// Exact fix-up after a speculative COLLECT pass (which quantized with the amax exported one step earlier), two kinds
+// of work over one persistent grid:
+//  1. an entry whose exported amax changes (exported_amax) is quantized again with the new amax over its live blocks
+//     [live_from, n_units) (live[2 i] = live_from, ops.live_block_ranges): the prefix below live_from is overwritten by
+//     later entries of the table that share the output buffer, and the live ranges of different entries never
+//     overlap.  Every CTA checks the entries 256 at a time (one per thread) and grid-strides over the range of each
+//     changed one; redo_count gets one increment each.
+//  2. pieces[3 p .. 3 p + 2] = (entry, from, to): the live blocks of the pre-flagged output tiles (ops.output_tiles),
+//     where live blocks of two entries meet, so that neither pass of the fused step can order all their stores; one
+//     CTA per piece.  It uses the exported amax too, so it writes what 1 writes where they meet.
+// Every other live block was stored last by the second pass of the fused step, after the first pass had completed.
 template <typename Tag, int VB, int UNROLL>
 __global__ void __launch_bounds__(kNvThreads)
     nvfp4_dyn_multi_fixup_kernel(const MultiDesc *__restrict__ descs, const unsigned long long *__restrict__ live,
                                  int n_desc, const uint32_t *__restrict__ slots, const void *__restrict__ amax_base,
-                                 int amax_dtype, int *__restrict__ redo_count) {
+                                 int amax_dtype, const long long *__restrict__ pieces, int n_pieces,
+                                 int *__restrict__ redo_count) {
   __shared__ uint32_t s_work[kNvThreads / 32];
   __shared__ float s_amax[kNvThreads];
-  __shared__ unsigned long long s_end[kNvThreads];
   pdl_launch_dependents();
   pdl_wait();
   const size_t stride = (size_t)gridDim.x * kNvThreads;
@@ -178,28 +214,9 @@ __global__ void __launch_bounds__(kNvThreads)
     const int e = e0 + (int)threadIdx.x;
     bool work = false;
     if (e < n_desc) {
-      const long long slot = descs[e].slot;
-      const float v = __uint_as_float(__ldcg(slots + slot));
-      uint32_t nb, ob;
-      float na;
-      if (amax_dtype == B200Q_F32) {
-        nb = __float_as_uint(v);
-        ob = static_cast<const uint32_t *>(amax_base)[slot];
-        na = v;
-      } else if (amax_dtype == B200Q_BF16) {
-        nb = f2bf_bits(v);
-        ob = static_cast<const uint16_t *>(amax_base)[slot];
-        na = __uint_as_float(nb << 16);
-      } else {
-        nb = f2h_bits(v);
-        ob = static_cast<const uint16_t *>(amax_base)[slot];
-        na = h2f_bits((uint16_t)nb);
-      }
-      const bool redo = nb != ob;
-      const unsigned long long end = redo ? descs[e].n_units : live[2 * e + 1];
-      work = end > live[2 * e];
-      s_amax[threadIdx.x] = na;
-      s_end[threadIdx.x] = end;
+      bool redo;
+      s_amax[threadIdx.x] = exported_amax(descs[e], slots, amax_base, amax_dtype, redo);
+      work = redo && descs[e].n_units > live[2 * e];
       if (redo && blockIdx.x == 0) atomicAdd(redo_count, 1);
     }
     const uint32_t ballot = __ballot_sync(0xffffffffu, work);
@@ -209,7 +226,7 @@ __global__ void __launch_bounds__(kNvThreads)
       for (uint32_t bits = s_work[w]; bits != 0u; bits &= bits - 1u) {
         const int k = w * 32 + __ffs((int)bits) - 1;
         const MultiDesc d = descs[e0 + k];
-        const size_t end = s_end[k];
+        const size_t end = d.n_units;
         DynScale ds;
         ds.setup(s_amax[k]);
         const ExactDiv d6(ds.six_gs);
@@ -217,20 +234,27 @@ __global__ void __launch_bounds__(kNvThreads)
           dyn_fq_blocks<Tag, VB, UNROLL, false>(d.x, d.y, i, stride, end, ds, d6);
       }
     }
-    __syncthreads();  // s_work / s_amax / s_end are refilled for the next 256 entries
+    __syncthreads();  // s_work / s_amax are refilled for the next 256 entries
+  }
+  for (int p = blockIdx.x; p < n_pieces; p += gridDim.x) {
+    const MultiDesc d = descs[pieces[3 * p]];
+    bool redo;
+    const float a = exported_amax(d, slots, amax_base, amax_dtype, redo);
+    cta_fq_range<Tag, VB, UNROLL>(d, (size_t)pieces[3 * p + 1], (size_t)pieces[3 * p + 2], a);
   }
 }
 
 template <typename Tag>
 static int launch_nvfp4_fixup(const MultiDesc *d, const unsigned long long *live, int n_desc, const uint32_t *slots,
-                              const void *amax_base, int amax_dtype, int *redo_count, cudaStream_t st) {
+                              const void *amax_base, int amax_dtype, const long long *pieces, int n_pieces,
+                              int *redo_count, cudaStream_t st) {
   auto kern = nvfp4_dyn_multi_fixup_kernel<Tag, 32, 2>;
   static int per_sm = 0;  // resident CTAs per SM: the grid is exactly one wave, so no CTA waits for another to finish
   if (per_sm == 0 && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kNvThreads, 0) != cudaSuccess)
     return check_launch("nvfp4_dyn_multi_fixup_kernel occupancy");
   const int grid = sm_count() * (per_sm < 1 ? 1 : per_sm);
   launch_pdl(kern, dim3((unsigned)grid), dim3(kNvThreads), 0, st, d, live, n_desc, slots, amax_base, amax_dtype,
-             redo_count);
+             pieces, n_pieces, redo_count);
   return check_launch("nvfp4_dyn_multi_fixup_kernel");
 }
 
@@ -635,18 +659,19 @@ int b200q_collect_fake_quant_nvfp4_multi(const void *descs, int n_desc, size_t t
 }
 
 int b200q_fake_quant_nvfp4_multi_fixup(const void *descs, const void *live, int n_desc, int dtype,
-                                       const float *slots, const void *amax_base, int amax_dtype, int *redo_count,
-                                       b200q_stream_t stream) {
+                                       const float *slots, const void *amax_base, int amax_dtype, const void *pieces,
+                                       int n_pieces, int *redo_count, b200q_stream_t stream) {
   if (n_desc == 0) return B200Q_OK;
   B200Q_REQUIRE(descs != nullptr && live != nullptr && slots != nullptr && amax_base != nullptr &&
-                    redo_count != nullptr && n_desc > 0,
+                    (pieces != nullptr || n_pieces == 0) && redo_count != nullptr && n_desc > 0 && n_pieces >= 0,
                 "null pointer");
   B200Q_REQUIRE(dtype_ok(amax_dtype), "unknown amax dtype %d", amax_dtype);
   const MultiDesc *d = static_cast<const MultiDesc *>(descs);
   const unsigned long long *lf = static_cast<const unsigned long long *>(live);
   const uint32_t *sl = reinterpret_cast<const uint32_t *>(slots);
+  const long long *pc = static_cast<const long long *>(pieces);
   B200Q_DISPATCH_DTYPE(dtype, Tag,
-                       return launch_nvfp4_fixup<Tag>(d, lf, n_desc, sl, amax_base, amax_dtype, redo_count,
+                       return launch_nvfp4_fixup<Tag>(d, lf, n_desc, sl, amax_base, amax_dtype, pc, n_pieces, redo_count,
                                                       (cudaStream_t)stream));
   return B200Q_OK;
 }

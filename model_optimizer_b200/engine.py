@@ -403,7 +403,7 @@ class ShardedPTQEngine:
     def act_bytes_per_step(self) -> tuple[int, int]:
         """(collect bytes, fake-quant bytes) of algorithmic HBM traffic for one batch on this rank.  ``grouped``: the
         collect rides on the fake-quant read, and the first item is the fix-up's traffic when no exported amax changes
-        (the contested output ranges it rewrites, ``ops.live_block_ranges``; known once captured)."""
+        (the live blocks of the pre-flagged output tiles it rewrites, ``ops.output_tiles``; known once captured)."""
         elems = sum(self.tokens * cin for _, _, cin in self.quantizers)
         es = torch.empty((), dtype=self.dtype).element_size()
         return self._fixup_bytes if self.grouped else elems * es, 2 * elems * es

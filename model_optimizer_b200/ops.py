@@ -151,6 +151,81 @@ def live_block_ranges(inputs, outputs, block_bytes: int) -> list[tuple[int, int]
     return ranges
 
 
+NVFP4_TILE_BLOCKS = 512                                # one CTA tile of the NVFP4 grids: 256 threads x 2 blocks
+
+
+def output_tiles(outputs, block_bytes: int, tile_blocks: int = NVFP4_TILE_BLOCKS):
+    """Store-order bookkeeping of the fused collect + fake quant over ``outputs`` (``(address, nbytes)`` per entry, the
+    layouts ``live_block_ranges`` accepts).  Outputs sharing a buffer are prefixes of it, so tile k (``tile_blocks``
+    blocks of ``block_bytes``) of every entry writing that buffer covers the same bytes.  Buffer tiles are numbered
+    buffer by buffer, in order of first use.  Returns ``(tile0, owner, expected, preflag, pieces)``:
+
+    - ``tile0[i]``: the number of entry i's tile 0;
+    - per buffer tile: ``owner``, the last entry writing any part of it (the one that leaves its first block);
+      ``expected``, the number of earlier entries writing any part of it; ``preflag``, whether live blocks of more
+      than one entry lie in it (a live bound inside the tile) -- its stores cannot be ordered by one check;
+    - ``pieces``: ``(entry, from, to)`` block ranges, the live blocks of each entry inside a pre-flagged tile."""
+    nblk = [n // block_bytes for _, n in outputs]
+    live_from, after = [0] * len(outputs), {}          # as in live_block_ranges
+    for i in range(len(outputs) - 1, -1, -1):
+        a = outputs[i][0]
+        live_from[i] = min(nblk[i], after.get(a, 0))
+        after[a] = max(after.get(a, 0), nblk[i])
+    bases = {}
+    for i, (a, _) in enumerate(outputs):
+        bases.setdefault(a, []).append(i)
+    first = {}
+    total = 0
+    for a, ents in bases.items():
+        first[a] = total
+        total += -(-max(nblk[i] for i in ents) // tile_blocks)
+    tile0 = [first[a] for a, _ in outputs]
+    owner, expected, n_live = [-1] * total, [0] * total, [0] * total
+    for a, ents in bases.items():
+        ns = sorted(nblk[i] for i in ents)
+        for k in range(-(-ns[-1] // tile_blocks)):
+            # entries writing any block of tile k: those with more than k * tile_blocks blocks
+            expected[first[a] + k] = len(ns) - bisect.bisect_right(ns, k * tile_blocks) - 1
+    for i, lf in enumerate(live_from):
+        if lf >= nblk[i]:
+            continue
+        t0, t1 = lf // tile_blocks, (nblk[i] - 1) // tile_blocks
+        for k in range(-(-lf // tile_blocks), t1 + 1):          # tiles whose first block entry i leaves
+            owner[tile0[i] + k] = i
+        for k in {t0, t1}:                                       # only a range's end tiles can hold other live blocks
+            n_live[tile0[i] + k] += 1
+    preflag = [c > 1 for c in n_live]
+    pieces = []
+    for i, lf in enumerate(live_from):
+        if lf >= nblk[i]:
+            continue
+        for k in sorted({lf // tile_blocks, (nblk[i] - 1) // tile_blocks}):
+            if preflag[tile0[i] + k]:
+                pieces.append((i, max(lf, k * tile_blocks), min(nblk[i], (k + 1) * tile_blocks)))
+    return tile0, owner, expected, preflag, pieces
+
+
+def second_pass_tiles(outputs, block_bytes: int, tile_blocks: int = NVFP4_TILE_BLOCKS) -> list[tuple[int, int]]:
+    """The two-pass order of the fused collect + fake quant over ``outputs`` (as for ``output_tiles``): per entry the
+    range ``[k_from, k_to)`` of its tiles that run in the SECOND pass -- the tiles it writes last while an earlier entry
+    writes them too.  Every other tile runs in the first pass.  The second pass starts after the first has completed,
+    and no two of its tiles cover the same bytes, so every tile ends with its last writer's stores; only the live
+    blocks of other entries inside a pre-flagged tile (``output_tiles``) can still end wrong, and the fix-up rewrites
+    them."""
+    tile0, owner, expected, _, _ = output_tiles(outputs, block_bytes, tile_blocks)
+    res = []
+    for i, (_, n) in enumerate(outputs):
+        n_tiles = -(-(n // block_bytes) // tile_blocks)
+        k = 0
+        while k < n_tiles and owner[tile0[i] + k] != i:      # the tiles an entry writes last are a suffix of its tiles
+            k += 1
+        k_to = k
+        while k_to < n_tiles and expected[tile0[i] + k_to] > 0:   # ... and those with earlier writers a prefix
+            k_to += 1
+        res.append((k, k_to))
+    return res
+
+
 class TensorTable:
     """Device descriptor table for the multi-tensor launches (``b200q_amax_per_tensor_multi`` /
     ``b200q_fake_quant_nvfp4_multi``): build once per set of (static) buffers, launch many times -- e.g. inside a
@@ -192,11 +267,32 @@ class TensorTable:
         self.live = None
         if fused:
             nb = [x.numel() * es for x in xs]
-            live = live_block_ranges([(x.data_ptr(), n) for x, n in zip(xs, nb)],
-                                     [(y.data_ptr(), n) for y, n in zip(ys, nb)], 16 * es)
+            outputs = [(y.data_ptr(), n) for y, n in zip(ys, nb)]
+            live = live_block_ranges([(x.data_ptr(), n) for x, n in zip(xs, nb)], outputs, 16 * es)
+            _, _, _, _, pieces = output_tiles(outputs, 16 * es)
             self.live = torch.tensor(live, dtype=torch.int64).to(self.device)
-            # bytes the fix-up moves when no amax changes: the contested ranges are read and written again
-            self.fixup_bytes = sum(c - f for f, c in live) * 16 * es * 2
+            # the fused step runs as two passes over sub-tensor descriptors of the same entries (second_pass_tiles)
+            tile_b = per_cta * 16 * es
+            passes = ([], [])
+            for (x, y, n_units, _, slot), (k0, k1) in zip(rows, second_pass_tiles(outputs, 16 * es)):
+                n_t = (n_units + per_cta - 1) // per_cta
+                for p, a, b in ((0, 0, k0), (1, k0, k1), (0, k1, n_t)):
+                    if b > a:
+                        passes[p].append([x + a * tile_b, y + a * tile_b, min(n_units, b * per_cta) - a * per_cta, 0,
+                                          slot])
+            self.passes = []
+            for r in passes:
+                first = 0
+                for row in r:
+                    row[3] = first
+                    first += (row[2] + per_cta - 1) // per_cta
+                if r:
+                    self.passes.append((torch.tensor(r, dtype=torch.int64).to(self.device), len(r), first))
+            self.n_pieces = len(pieces)
+            self.pieces = torch.tensor(pieces or [(0, 0, 0)], dtype=torch.int64).to(self.device)
+            # bytes the fix-up moves when no amax changes: the live blocks of the pre-flagged tiles are read and
+            # written again
+            self.fixup_bytes = sum(b - a for _, a, b in pieces) * 16 * es * 2
         self._keep = (list(xs), None if ys is None else list(ys))  # the table holds raw pointers
 
 
@@ -229,27 +325,29 @@ def _fused_args(table: TensorTable, slots: torch.Tensor, amax_base: torch.Tensor
 def collect_fake_quant_nvfp4_multi(table: TensorTable, slots: torch.Tensor, amax_base: torch.Tensor):
     """``fake_quant_nvfp4_multi(table, amax_base)`` and ``amax_per_tensor_multi_(slots, table)`` in ONE read of every
     input: the outputs are SPECULATIVE (quantized with the amax ``amax_base`` holds now, i.e. the previous export) until
-    ``fake_quant_nvfp4_multi_fixup`` has run.  ``table``: built with ``fused=True``."""
+    ``fake_quant_nvfp4_multi_fixup`` has run.  ``table``: built with ``fused=True``.  Two launches in stream order
+    (``second_pass_tiles``): the second stores the tiles that entries sharing an output buffer write last."""
     _fused_args(table, slots, amax_base)
     with torch.cuda.device(table.device):
-        call("b200q_collect_fake_quant_nvfp4_multi", table.table.data_ptr(), table.n, table.total_ctas,
-             _DT[table.dtype], slots.data_ptr(), amax_base.data_ptr(), _DT[amax_base.dtype],
-             torch.cuda.current_stream(table.device).cuda_stream)
+        for descs, n, total_ctas in table.passes:
+            call("b200q_collect_fake_quant_nvfp4_multi", descs.data_ptr(), n, total_ctas, _DT[table.dtype],
+                 slots.data_ptr(), amax_base.data_ptr(), _DT[amax_base.dtype],
+                 torch.cuda.current_stream(table.device).cuda_stream)
 
 
 def fake_quant_nvfp4_multi_fixup(table: TensorTable, slots: torch.Tensor, amax_base: torch.Tensor,
                                  redo_count: torch.Tensor):
     """Between ``collect_fake_quant_nvfp4_multi`` and the export of ``slots`` into ``amax_base``: redo, with the new
-    amax, the entries whose exported amax is about to change, and rewrite the contested part of every live output range
-    (``live_block_ranges``), so that after the export everything is bit-identical to collect -> export -> fake quant.
-    ``redo_count`` (int32 CUDA scalar) += number of entries redone."""
+    amax, the live output range (``live_block_ranges``) of every entry whose exported amax is about to change, and
+    rewrite the live blocks of the pre-flagged output tiles (``output_tiles``), so that after the export everything is
+    bit-identical to collect -> export -> fake quant.  ``redo_count`` (int32 CUDA scalar) += number of entries redone."""
     _fused_args(table, slots, amax_base)
     if redo_count.dtype != torch.int32 or not redo_count.is_cuda or redo_count.numel() != 1:
         raise B200QuantError("redo_count must be an int32 CUDA tensor of one element")
     with torch.cuda.device(table.device):
         call("b200q_fake_quant_nvfp4_multi_fixup", table.table.data_ptr(), table.live.data_ptr(), table.n,
-             _DT[table.dtype], slots.data_ptr(), amax_base.data_ptr(), _DT[amax_base.dtype], redo_count.data_ptr(),
-             torch.cuda.current_stream(table.device).cuda_stream)
+             _DT[table.dtype], slots.data_ptr(), amax_base.data_ptr(), _DT[amax_base.dtype], table.pieces.data_ptr(),
+             table.n_pieces, redo_count.data_ptr(), torch.cuda.current_stream(table.device).cuda_stream)
 
 
 def hist_plan_(plan_state: torch.Tensor, batch_amax: torch.Tensor, nbins0: int, capacity: int) -> torch.Tensor:

@@ -71,6 +71,12 @@ def run():
     amax2.copy_(slots2)
     assert torch.equal(slots2, slots) and int(redo) == 2, "fused collect mismatch"
     assert all(torch.equal(a, b) for a, b in zip(ys2, ys)), "fused fake quant mismatch"
+    # two entries sharing one output buffer: the second one's stores must be what the buffer keeps
+    yb = torch.empty_like(x)
+    t_ring = ops.TensorTable(xs, None, [yb, yb], "block16", fused=True)
+    ops.collect_fake_quant_nvfp4_multi(t_ring, slots2, amax2)
+    ops.fake_quant_nvfp4_multi_fixup(t_ring, slots2, amax2, redo)
+    assert torch.equal(yb, ys[1]) and int(redo) == 2, "fused fake quant into a shared buffer mismatch"
     from .calib import HistogramCalibrator
 
     hc = HistogramCalibrator(8, None, False, num_bins=512)
