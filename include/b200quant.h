@@ -417,6 +417,27 @@ int b200q_fake_quant_nvfp4_rotated(const void *x, void *y, int dtype, size_t n_r
                                    size_t block_size, int rotate_back, const void *global_amax, int amax_dtype,
                                    b200q_stream_t stream);
 
+/* ---- (5) GPTQ weight calibration ------------------------------------------------------------ */
+
+/* The column loop of one GPTQ block (gptq_blockwise_update, quantization/utils/calib_utils.py:241-276) on the fp32
+ * working matrix.  w: [rows, ldw] fp32, w[0] is the block's first column (global column col0); its nb <= 128 columns
+ * are replaced by the fake-quantized values.  u: [nb, ldu] fp32, the block of the upper Cholesky factor of the
+ * inverse Hessian (upper triangle read).  e: [rows, nb] fp32 out, the scaled errors.  For i = 0 .. nb-1:
+ *   q = Q(w_i); w_i := q; err = (w_i - q) / u[i,i]; w_j = w_j + fl(-err * u[i,j]) for j >= i; e[:, i] = err
+ * (the product rounded, then added: the arithmetic of ATen's CUDA addr_).  Q by fmt:
+ *   0 integer (num_bits, is_unsigned, narrow_range; b200q_fake_quant_int), 1 FP8-E4M3 (448 / amax;
+ *   b200q_fake_quant_fp8): amax[row * amax_row_stride + (col0 + c) / amax_col_block] in amax_dtype
+ *   (per tensor: stride 0 and a column block beyond the matrix; per row: stride 1);
+ *   2 NVFP4 static (b200q_fake_quant_nvfp4_static, fp8_max_norm 448): fp32 block amax indexed the same way with
+ *   amax_col_block 16, fp32 global_amax[0];
+ *   3 NVFP4 dynamic (b200q_fake_quant_nvfp4): amax[0] is the per-tensor amax, the 16-element block amax is taken
+ *   over the current working values at every column.
+ * NVFP4 needs nb % 16 == 0 and col0 % 16 == 0.  No NaN / inf special case beyond the quantizers' own rules. */
+int b200q_gptq_block(float *w, size_t ldw, size_t rows, int nb, const float *u, size_t ldu, float *e, int fmt,
+                     const void *amax, int amax_dtype, size_t amax_row_stride, size_t amax_col_block, size_t col0,
+                     int num_bits, int is_unsigned, int narrow_range, const float *global_amax,
+                     b200q_stream_t stream);
+
 /* ---- self tests (device-side numerics used by tests/, not by the product path) ----------- */
 /* Checks the hoisted-reciprocal exact division against div.rn.f32 on n pseudo-random pairs
  * (seeded); returns the number of mismatches in *mismatches_host. */

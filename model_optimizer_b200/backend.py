@@ -23,6 +23,11 @@ SURVEY.md 8(b), plus the module-level functions the hooks cannot reach.
    * ``normalized_hadamard_transform`` as named in ``nn/modules/tensor_quantizer.py`` (:67, called by
      ``_rotate_inputs`` :664-668): every ``rotate`` config on CUDA tensors runs ``b200q_hadamard`` instead of needing
      the external ``fast_hadamard_transform`` package (other inputs go to the host application's own function).
+6. ``register_gptq_helper("b200", B200GPTQHelper)`` (utils/calib_utils.py:316-326): ``gptq`` builds this
+   ``GPTQHelper`` subclass for weight quantizers on the b200 backend.  Its ``_blockwise_update`` runs the GPTQ column
+   kernel (``b200q_gptq_block``, one launch per block, plus the reference's trailing ``addmm_``) for the formats the
+   kernel covers, and the reference's own loop for everything else.  The reference's ``layerwise_calibrate`` thus
+   gives layerwise GPTQ on the kernel.  Like the backend registration, it stays in place after ``uninstall()``.
 
 Nothing here is imported by the engine itself; ``install()`` raises if modelopt is absent.
 ``stats`` counts kernel-path calls per hook so a test can prove which side executed.
@@ -274,8 +279,26 @@ def _make_mse_factory(base, ref_mse_cls):
     return B200MseCalibrator
 
 
+def _make_gptq_helper(ref_helper_cls):
+    class B200GPTQHelper(ref_helper_cls):
+        """``GPTQHelper`` whose blockwise update runs ``ops.gptq_blockwise_update`` for quantizers inside the GPTQ
+        kernel's scope (the unfused semantics of ``gptq_blockwise_update`` for every covered format, whatever
+        ``fused`` says); other quantizers, and CPU weights, run the host application's own loop."""
+
+        def _blockwise_update(self, block_size):
+            q = self.module.weight_quantizer
+            w = self.weight
+            desc = ops.gptq_quantizer_desc(q, w.shape, block_size, w.device) if w.is_cuda else None
+            if desc is None:
+                return super()._blockwise_update(block_size)
+            stats["gptq.block"] += 1
+            ops.gptq_blockwise_update(self.weight, self.h_inv, block_size, q, desc=desc)
+
+    return B200GPTQHelper
+
+
 def install(patch_extensions: bool = True, patch_functions: bool = True):
-    """Register the backend, the calibrator classes, the FP8-sweep factory and (optionally) the extension shims
+    """Register the backend, the calibrator classes, the FP8-sweep factory, the GPTQ helper and (optionally) the extension shims
     and function rebinds in modelopt.  Returns ``(B200MaxCalibrator, B200HistogramCalibrator)``."""
     import modelopt.torch.quantization.calib as ref_calib
     import modelopt.torch.quantization.extensions as ref_ext
@@ -307,6 +330,11 @@ def install(patch_extensions: bool = True, patch_functions: bool = True):
     ref_calib.B200MaxCalibrator = B200MaxCalibrator
     ref_calib.B200HistogramCalibrator = B200HistogramCalibrator
     ref_model_calib._register_fp8_sweep_calibrator("b200", lambda amax, axis, quant_func: sweep_cls(amax, axis, quant_func))
+    import modelopt.torch.quantization.utils.calib_utils as ref_calib_utils
+
+    if "gptq" not in _saved:
+        _saved["gptq"] = _make_gptq_helper(ref_calib_utils.GPTQHelper)
+    ref_calib_utils.register_gptq_helper("b200", _saved["gptq"])
 
     if patch_extensions and "ext" not in _saved:
         _saved["ext"] = {(m, n): getattr(m, n) for m in (ref_ext, ref_tensor_quant)

@@ -83,6 +83,46 @@ class QuantizerAttributeConfig:
             raise ValueError(f"rotate must be a bool, a dict or a RotateConfig, got {self.rotate!r}")
 
 
+@dataclass
+class GPTQCalibConfig:
+    """quantization/config.py:1204-1250: GPTQ (second-order blockwise weight update).  ``perc_damp`` in (0, 1] is the
+    fraction of the mean Hessian diagonal added as damping; ``block_size`` columns per GPTQ block; ``fused`` is
+    accepted for parity (the engine's kernel implements the unfused semantics for every format it covers).
+    ``layerwise``: a bool or ``{"enable": ...}``; layer-by-layer calibration is not part of the engine's own API, so
+    ``enable: true`` is refused at calibration time (the drop-in into the reference provides it).  ``None`` for
+    ``perc_damp`` / ``block_size`` is accepted like the reference's config and means the default."""
+
+    method: str = "gptq"
+    perc_damp: float | None = 0.01
+    block_size: int | None = 128
+    fused: bool = False
+    layerwise: bool | dict | None = None
+
+    def __post_init__(self):
+        if self.method != "gptq":
+            raise ValueError(f"method must be 'gptq', got {self.method!r}")
+        if self.perc_damp is None:
+            self.perc_damp = 0.01
+        if self.block_size is None:
+            self.block_size = 128
+        p = self.perc_damp
+        if isinstance(p, bool) or not isinstance(p, (int, float)) or not (0.0 < p <= 1.0):
+            raise ValueError(f"perc_damp must be in (0, 1], got {p!r}")
+        b = self.block_size
+        if isinstance(b, bool) or not isinstance(b, int) or b <= 0:
+            raise ValueError(f"block_size must be a positive int, got {b!r}")
+        if not isinstance(self.fused, bool):
+            raise ValueError(f"fused must be a bool, got {self.fused!r}")
+        lw = self.layerwise
+        if lw is not None and not isinstance(lw, (bool, dict)):
+            raise ValueError(f"layerwise must be a bool or a dict, got {lw!r}")
+
+    @property
+    def layerwise_enabled(self) -> bool:
+        lw = self.layerwise
+        return bool(lw.get("enable", False)) if isinstance(lw, dict) else bool(lw)
+
+
 _DEFAULT_DISABLED = [
     "*block_sparse_moe.gate*", "*linear_attn.conv1d*", "*linear_attn.in_proj_a*", "*linear_attn.in_proj_b*",
     "*lm_head*", "*mixer.conv1d*", "*mlp.gate.*", "*mlp.shared_expert_gate.*", "*output_layer*", "*proj_out.*",
@@ -168,4 +208,4 @@ def get_preset(name: str) -> dict:
     return copy.deepcopy(PRESETS[name])
 
 
-__all__ = ["QuantizerAttributeConfig", "RotateConfig", "PRESETS", "get_preset", *PRESETS.keys()]
+__all__ = ["QuantizerAttributeConfig", "RotateConfig", "GPTQCalibConfig", "PRESETS", "get_preset", *PRESETS.keys()]

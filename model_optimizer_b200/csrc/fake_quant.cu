@@ -5,7 +5,7 @@
 // Reference semantics (bit-exact):
 //   integer : kernels/quantization/gemm/tensor_quant_gpu.cu:43-140  (fake_tensor_quant_device)
 //   fp8     : kernels/quantization/gemm/tensor_quant_gpu_fp8.cu:36-107 (fake_e4m3fy[_with_axis])
-#include "common.cuh"
+#include "intq.cuh"
 
 namespace b200q {
 
@@ -113,28 +113,6 @@ struct IntScale {
     }
   }
   __device__ __forceinline__ float apply(float x) const { return apply_ref(x); }
-};
-
-// ---------------------------------------------------------------------------------------------
-// fp8 op
-// ---------------------------------------------------------------------------------------------
-struct Fp8Scale {
-  float scale, inv;
-  // eager == false: the CUDA extension's rule, scale = 448.f / amax (IEEE division, tensor_quant_gpu_fp8.cu:94-98)
-  // eager == true : _fp8_eager's rule (tensor_quant.py:46-59), where `448.0 / safe_amax` is torch's
-  //                 Tensor.__rtruediv__ = safe_amax.reciprocal() * 448.0 (two roundings); used by the reference
-  //                 whenever amax has more than one non-singleton dim (2-D block scales) and on CPU
-  __device__ __forceinline__ void setup(float amax, bool eager = false) {
-    const float safe = (amax <= (1.0f / (1 << 24))) ? 1.0f : amax;
-    scale = eager ? __fmul_rn(__frcp_rn(safe), 448.0f) : __fdiv_rn(448.0f, safe);
-    inv = __fdiv_rn(1.0f, scale);
-  }
-  __device__ __forceinline__ void apply2(float &a, float &b) const {
-    float lo, hi;
-    e4m3x2_to_f32x2(f32x2_to_e4m3x2(__fmul_rn(a, scale), __fmul_rn(b, scale)), lo, hi);
-    a = __fmul_rn(lo, inv);
-    b = __fmul_rn(hi, inv);
-  }
 };
 
 // plain torch-style cast round trip (amax == None): overflow -> NaN

@@ -339,28 +339,6 @@ static int launch_nvfp4_dyn(const void *x, void *y, size_t n_rows, size_t row_le
 // ---------------------------------------------------------------------------------------------
 // static fake quant: calibrated per-block amax (fp4_kernel.py:217-316)
 // ---------------------------------------------------------------------------------------------
-struct StaticScale {
-  bool quantize;
-  float sc, inv;  // fake_e4m3fy operands for the block-scale round trip
-  __device__ __forceinline__ void setup(const float *global_amax, int quantize_, float ratio) {
-    quantize = quantize_ != 0;
-    sc = inv = 1.0f;
-    if (quantize) {
-      // scale_fp8_quant_amax = global_amax * (448 / fp8_max_norm) / 6   (fp4_kernel.py:248)
-      const float qa = __fdiv_rn(__fmul_rn(global_amax[0], ratio), 6.0f);
-      // fake_e4m3fy (tensor_quant_gpu_fp8.cu:90-98)
-      const float safe = (qa <= (1.0f / (1 << 24))) ? 1.0f : qa;
-      sc = __fdiv_rn(448.0f, safe);
-      inv = __fdiv_rn(1.0f, sc);
-    }
-  }
-  __device__ __forceinline__ float block_scale(float amax_b) const {
-    float s = __fdiv_rn(amax_b, 6.0f);
-    if (quantize) s = __fmul_rn(e4m3_round(__fmul_rn(s, sc)), inv);
-    return s;
-  }
-};
-
 template <typename Tag, int VB, int UNROLL>
 __global__ void __launch_bounds__(kNvThreads)
     nvfp4_static_kernel(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t n_blocks,

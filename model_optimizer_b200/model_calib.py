@@ -14,6 +14,7 @@ B200-first differences (results identical, work removed):
 
 from __future__ import annotations
 
+import collections
 import warnings
 from typing import Callable
 
@@ -550,6 +551,144 @@ def awq_clip(model: nn.Module, forward_loop: Callable, max_co_batch_size: int = 
     _finalize_static_nvfp4(model)
 
 
+# ---- GPTQ ------------------------------------------------------------------------------------------
+# weight updates per path of gptq_blockwise_update: "gptq.kernel" (the column kernel) and "gptq.composed"
+stats: collections.Counter = collections.Counter()
+
+
+def update_hessian(input, hessian, n_samples):
+    """utils/calib_utils.py:50-77: running mean of ``2 X X^T`` over tokens; the same torch ops in the same order.
+    Zero tokens (an MoE expert that received none) return ``hessian`` itself unchanged."""
+    import math
+
+    input_flat = input.reshape(-1, input.shape[-1]).t().float()
+    batch_size = input_flat.shape[1]
+    if batch_size == 0:
+        return hessian, n_samples
+    hessian *= n_samples / (n_samples + batch_size)
+    n_samples += batch_size
+    scaled_input = math.sqrt(2 / n_samples) * input_flat
+    hessian.add_((scaled_input @ scaled_input.t()).to(hessian.device))
+    return hessian, n_samples
+
+
+def compute_hessian_inverse(hessian, weight, perc_damp):
+    """utils/calib_utils.py:80-113: upper Cholesky factor of the damped inverse Hessian.  Columns that are all zero in
+    ``weight`` are zeroed in the Hessian (diagonal 1); a Hessian that is not positive definite gives the identity,
+    with a warning."""
+    h = hessian.clone()
+    zero_cols = torch.nonzero(weight.eq(0).all(dim=0)).unsqueeze(-1)
+    h[zero_cols, :] = 0
+    h[:, zero_cols] = 0
+    h[zero_cols, zero_cols] = 1
+    damp = perc_damp * torch.mean(torch.diag(h))
+    diag_indices = torch.arange(h.shape[0], device=h.device)
+    h[diag_indices, diag_indices] += damp
+    try:
+        h = torch.cholesky_inverse(torch.linalg.cholesky(h))
+        return torch.linalg.cholesky(h, upper=True)
+    except (RuntimeError, torch.linalg.LinAlgError):
+        warnings.warn("Hessian is not positive definite, using identity matrix")
+        return torch.eye(h.shape[0], device=h.device, dtype=h.dtype)
+
+
+def gptq_blockwise_update_composed(weight, h_inv, block_size, quantize_fn):
+    """utils/calib_utils.py:241-276 as written: per column, fake-quantize the whole working matrix with
+    ``quantize_fn`` and keep one column, then a rank-1 ``addr_``.  Used for quantizers outside the GPTQ kernel's scope,
+    and by tests as the reference on the GPU."""
+    num_cols = weight.shape[1]
+    for block_start in range(0, num_cols, block_size):
+        block_end = min(block_start + block_size, num_cols)
+        n_cols_blk = block_end - block_start
+        h_inv_cho_blk = h_inv[block_start:block_end, block_start:block_end]
+        wblk = weight.clone()
+        errs = torch.zeros_like(weight[:, block_start:block_end])
+        for i in range(n_cols_blk):
+            w_ci = wblk[:, block_start + i]
+            d = h_inv_cho_blk[i, i]
+            qdq = quantize_fn(wblk)
+            weight[:, block_start + i] = qdq[:, block_start + i]
+            err = (w_ci - qdq[:, block_start + i]) / d
+            wblk[:, block_start + i: block_end].addr_(err, h_inv_cho_blk[i, i:], alpha=-1)
+            errs[:, i] = err
+        weight[:, block_end:].addmm_(errs, h_inv[block_start:block_end, block_end:], alpha=-1)
+
+
+def gptq_blockwise_update(weight, h_inv, block_size, quantizer) -> bool:
+    """GPTQ update of the fp32 working ``weight`` in place: the column kernel (``ops.gptq_blockwise_update``) when the
+    quantizer is inside its scope, else the composed loop.  Returns whether the kernel ran; ``stats`` counts both."""
+    desc = ops.gptq_quantizer_desc(quantizer, weight.shape, block_size, weight.device) if weight.is_cuda else None
+    if desc is not None:
+        ops.gptq_blockwise_update(weight, h_inv, block_size, quantizer, desc=desc)
+        stats["gptq.kernel"] += 1
+        return True
+    stats["gptq.composed"] += 1
+    gptq_blockwise_update_composed(weight, h_inv, block_size, quantizer)
+    return False
+
+
+@torch.no_grad()
+def gptq(model: nn.Module, forward_loop: Callable | None = None, perc_damp: float = 0.01, block_size: int = 128,
+         fused: bool = False, layerwise=None):
+    """model_calib.py:2191-2271 (non-layerwise): ``max_calibrate`` (static NVFP4 promotion and shared global amax
+    included), one forward that accumulates ``2 X X^T`` per quantized linear with an enabled weight quantizer (X is
+    the input quantizer's output when that quantizer is enabled; weight quantizers are disabled during this pass),
+    then per module the blockwise update of ``weight.float()`` with the inverse Hessian, written back in the weight's
+    dtype.  ``fused`` is accepted for config parity: the kernel implements the unfused semantics."""
+    from .config import GPTQCalibConfig
+
+    cfg = GPTQCalibConfig(perc_damp=perc_damp, block_size=block_size, fused=fused, layerwise=layerwise)
+    if cfg.layerwise_enabled:
+        raise NotImplementedError(
+            "gptq: layerwise calibration is not part of model_optimizer_b200's own API; run the reference's "
+            "mtq.quantize under model_optimizer_b200.backend.install(), whose layerwise_calibrate drives the GPTQ "
+            "kernel through the registered 'b200' GPTQ helper")
+    max_calibrate(model, forward_loop)
+    layers = [(n, m) for n, m in model.named_modules() if is_quantized_linear(m) and m.weight_quantizer.is_enabled]
+    if not layers:
+        warnings.warn("No quantized linear layers found, skipping GPTQ")
+        return
+    state = {}
+    for name, m in layers:
+        state[name] = [torch.zeros(m.weight.shape[-1], m.weight.shape[-1], dtype=torch.float32,
+                                   device=m.weight.device), 0]
+
+    def make_hook(name):
+        def hook(lin, args):
+            if not args:
+                return
+            inp = args[0]
+            iq = lin.input_quantizer
+            x = iq(inp) if iq is not None and iq.is_enabled else inp
+            st = state[name]
+            st[0], st[1] = update_hessian(x, st[0], st[1])
+        return hook
+
+    handles = [m.register_forward_pre_hook(make_hook(name)) for name, m in layers]
+    held = [q for n, q in _quantizers(model) if n.endswith("weight_quantizer") and q.is_enabled]
+    for q in held:                      # set_quantizer_by_cfg_context(*weight_quantizer: enable False)
+        q.disable()
+    try:
+        if forward_loop is not None:
+            forward_loop(model)
+    finally:
+        for h in handles:
+            h.remove()
+        for q in held:
+            q.enable()
+    for name, m in layers:
+        hessian = state[name][0].to(m.weight.device)
+        weight = m.weight.data.float().clone()
+        h_inv = compute_hessian_inverse(hessian, weight, cfg.perc_damp)
+        gptq_blockwise_update(weight, h_inv, cfg.block_size, m.weight_quantizer)
+        m.weight.data = weight.reshape(m.weight.shape).to(m.weight.data.dtype)
+        if hasattr(m, "invalidate_weight_cache"):
+            m.invalidate_weight_cache()
+        state[name] = None
+
+
 __all__ = ["max_calibrate", "mse_calibrate", "local_hessian_calibrate", "find_shared_weight_groups", "SHARED_PATTERNS", "smoothquant", "awq_lite", "awq_clip", "enable_stats_collection",
+           "gptq", "update_hessian", "compute_hessian_inverse", "gptq_blockwise_update",
+           "gptq_blockwise_update_composed",
            "finish_stats_collection", "weight_only_quantize", "apply_pre_quant_scale_and_smooth",
            "get_weight_scale", "get_scale"]

@@ -68,6 +68,7 @@ def calibrate(model: nn.Module, algorithm="max", forward_loop: Callable | None =
         "awq_clip": model_calib.awq_clip,
         "mse": model_calib.mse_calibrate,
         "local_hessian": model_calib.local_hessian_calibrate,
+        "gptq": model_calib.gptq,
     }.get(algorithm)
     if fn is None:
         raise ValueError(f"Unsupported calibration algorithm: {algorithm}")

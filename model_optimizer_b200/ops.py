@@ -901,6 +901,137 @@ def nvfp4_fp8_scale_sweep(w, global_amax, candidates="device", hessian=None):
     return best
 
 
+# ------------------------------------------------------------------------------------------------
+# GPTQ weight calibration
+# ------------------------------------------------------------------------------------------------
+GPTQ_INT, GPTQ_FP8, GPTQ_NVFP4_STATIC, GPTQ_NVFP4_DYNAMIC = 0, 1, 2, 3
+GPTQ_PER_TENSOR_COL_BLOCK = 1 << 62      # an amax column block wider than any matrix: one amax per row / tensor
+
+
+def _rows_view(t: torch.Tensor, name: str) -> torch.Tensor:
+    if not t.is_cuda or t.dtype != torch.float32 or t.dim() != 2 or t.stride(1) != 1:
+        raise B200QuantError(f"{name} must be a 2-D float32 CUDA tensor with unit column stride")
+    return t
+
+
+def gptq_block_update(w, u, fmt, amax, amax_row_stride=0, amax_col_block=GPTQ_PER_TENSOR_COL_BLOCK, col0=0,
+                      num_bits=8, unsigned=False, narrow_range=False, global_amax=None):
+    """The column loop of one GPTQ block (``b200q_gptq_block``): ``w`` [rows, nb] fp32 (a column slice of the working
+    matrix, row stride free) is replaced in place by its fake-quantized columns; ``u`` [nb, nb] fp32 is the block of
+    the upper Cholesky factor of the inverse Hessian (any strides: a column-major block is copied, nb x nb floats).
+    Returns the scaled errors E [rows, nb] (fp32)."""
+    _rows_view(w, "w")
+    if u.is_cuda and u.dtype == torch.float32 and u.dim() == 2 and u.stride(1) != 1:
+        u = u.contiguous()           # the factor of torch.linalg.cholesky(upper=True) is column-major
+    _rows_view(u, "u")
+    rows, nb = w.shape
+    if u.shape[0] < nb or u.shape[1] < nb:
+        raise B200QuantError(f"u {tuple(u.shape)} is smaller than the block ({nb} columns)")
+    amax = _prep(amax, "amax")
+    _dt(amax)
+    g = None
+    if global_amax is not None:
+        g = _prep(global_amax.reshape(-1), "global_amax")
+        if g.dtype != torch.float32:
+            raise B200QuantError("global_amax must be float32")
+    e = torch.empty(rows, nb, dtype=torch.float32, device=w.device)
+    call("b200q_gptq_block", w.data_ptr(), w.stride(0), rows, nb, u.data_ptr(), u.stride(0), e.data_ptr(), int(fmt),
+         amax.data_ptr(), _dt(amax), int(amax_row_stride), int(amax_col_block), int(col0), int(num_bits),
+         int(bool(unsigned)), int(bool(narrow_range)), None if g is None else g.data_ptr(), _stream(w))
+    return e
+
+
+def gptq_quantizer_desc(quantizer, shape, block_size=None, device=None) -> dict | None:
+    """The ``gptq_block_update`` description of a calibrated weight quantizer for a [out, in] weight, or None when
+    its fake quant is outside the kernel's scope (MX, 2-D blocks, NF4, pre_quant_scale, rotation, bias, padded block
+    layouts, NVFP4 blocks straddling GPTQ blocks of ``block_size`` columns, calibrated state on another device than
+    ``device``, or no calibrated ``_amax``: a dynamic per-tensor amax is taken over the whole working matrix at every
+    column).  Reads attributes that the engine's and the reference's quantizers share."""
+    desc = _gptq_quantizer_desc(quantizer, shape)
+    if desc is None:
+        return None
+    if block_size is not None and desc["fmt"] in (GPTQ_NVFP4_STATIC, GPTQ_NVFP4_DYNAMIC) and block_size % 16:
+        return None
+    if device is not None and any(isinstance(t, torch.Tensor) and t.device != torch.device(device)
+                                  for t in (desc["amax"], desc.get("global_amax"))):
+        return None
+    return desc
+
+
+def _gptq_quantizer_desc(quantizer, shape):
+    out_f, in_f = int(shape[0]), int(shape[1])
+    q = quantizer
+    if getattr(q, "_disabled", False) or not getattr(q, "_fake_quant", True) or getattr(q, "_lsq", False):
+        return None
+    if getattr(q, "pre_quant_scale", None) is not None or getattr(q, "rotate_is_enabled", False) \
+            or getattr(q, "bias", None) or getattr(q, "is_mx_format", False):
+        return None
+    amax = getattr(q, "_amax", None)
+    if not isinstance(amax, torch.Tensor) or not amax.is_cuda or amax.dtype not in _DT:
+        return None
+    nbits = q._num_bits
+    bs = q._block_sizes
+    if bs:
+        keys = [k for k in bs if isinstance(k, int)]
+        if len(keys) != 1 or keys[0] not in (-1, 1) or bs[keys[0]] is None or bs.get("four_over_six", False) \
+                or bs.get("scale_block_sizes"):
+            return None
+        cb = int(bs[keys[0]])
+        if in_f % cb:
+            return None
+        scale_bits = bs.get("scale_bits")
+        if bs.get("type", "static") == "dynamic":
+            if nbits == (2, 1) and scale_bits == (4, 3) and cb == 16 and amax.numel() == 1:
+                return {"fmt": GPTQ_NVFP4_DYNAMIC, "amax": amax}
+            return None
+        if nbits == (2, 1):
+            g = getattr(q, "_global_amax", None)
+            if scale_bits == (4, 3) and cb == 16 and isinstance(g, torch.Tensor) and g.numel() == 1 \
+                    and amax.numel() == out_f * in_f // 16:
+                return {"fmt": GPTQ_NVFP4_STATIC, "amax": amax.float(), "amax_row_stride": in_f // 16,
+                        "amax_col_block": 16, "global_amax": g.float()}
+            return None
+        if scale_bits is not None or (isinstance(nbits, tuple) and nbits != (4, 3)) \
+                or amax.numel() != out_f * in_f // cb:
+            return None
+        desc = {"amax": amax, "amax_row_stride": in_f // cb, "amax_col_block": cb}
+    elif isinstance(nbits, tuple) and nbits != (4, 3):
+        return None
+    elif amax.numel() == 1:
+        desc = {"amax": amax}
+    elif amax.dim() == 2 and tuple(amax.shape) == (out_f, 1):
+        desc = {"amax": amax, "amax_row_stride": 1}
+    else:
+        return None
+    if nbits == (4, 3):
+        desc["fmt"] = GPTQ_FP8
+    else:
+        desc.update(fmt=GPTQ_INT, num_bits=nbits, unsigned=q._unsigned, narrow_range=q._narrow_range)
+    return desc
+
+
+def gptq_blockwise_update(weight, h_inv, block_size, quantizer, desc=None):
+    """``gptq_blockwise_update`` (utils/calib_utils.py:241-276) with the column loop of every block in one kernel:
+    ``weight`` [out, in] fp32 is updated in place; per block, ``gptq_block_update`` then the reference's trailing
+    ``weight[:, be:].addmm_(E, h_inv[bs:be, be:], alpha=-1)`` (a cuBLAS GEMM through torch).  Raises for a quantizer
+    outside the kernel's scope (``gptq_quantizer_desc`` is None); callers take the composed loop there."""
+    if desc is None:
+        desc = gptq_quantizer_desc(quantizer, weight.shape, block_size, weight.device)
+    if desc is None:
+        raise B200QuantError("gptq_blockwise_update: the weight quantizer is outside the GPTQ kernel's scope")
+    if desc["fmt"] in (GPTQ_NVFP4_STATIC, GPTQ_NVFP4_DYNAMIC) and block_size % 16:
+        raise B200QuantError(f"gptq_blockwise_update: NVFP4 blocks straddle GPTQ blocks of {block_size} columns")
+    _rows_view(weight, "weight")
+    if not h_inv.is_cuda or h_inv.dtype != torch.float32 or h_inv.dim() != 2:
+        raise B200QuantError("h_inv must be a 2-D float32 CUDA tensor")
+    num_cols = weight.shape[1]
+    for bs in range(0, num_cols, block_size):
+        be = min(bs + block_size, num_cols)
+        errs = gptq_block_update(weight[:, bs:be], h_inv[bs:be, bs:be], col0=bs, **desc)
+        weight[:, be:].addmm_(errs, h_inv[bs:be, be:], alpha=-1)
+    return weight
+
+
 def selftest_fastdiv(seed: int, n: int) -> int:
     import ctypes
 

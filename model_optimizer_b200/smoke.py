@@ -107,6 +107,18 @@ def run():
     assert float((rr.float() - x.float()).abs().max()) <= 2 ** -6 * float(x.float().abs().max()), "rotation round trip"
     fused = ops.fake_quant_nvfp4_rotated(x, 128, rs.to(torch.bfloat16), True)
     assert torch.equal(fused, ops.hadamard(ops.fake_quant_nvfp4(r, rs.to(torch.bfloat16)), 128)), "rotated NVFP4 mismatch"
+    # (7) one GPTQ block (NVFP4 dynamic weights, 128 columns) against the C oracle
+    from tools import gptq_oracle
+
+    gw = x[:64, :128].float().contiguous() * 0.05
+    gx = torch.randn(512, 128, device="cuda", generator=g, dtype=torch.float64)
+    gu = torch.linalg.cholesky(torch.cholesky_inverse(torch.linalg.cholesky(gx.T @ gx / 512)), upper=True).float()
+    gamax = gw.abs().amax().reshape(1).to(torch.bfloat16)
+    want_w, want_e = gptq_oracle.gptq_block(gw.cpu().numpy(), gu.cpu().numpy(), ops.GPTQ_NVFP4_DYNAMIC,
+                                            gamax.float().cpu().numpy())
+    ge = ops.gptq_block_update(gw, gu, ops.GPTQ_NVFP4_DYNAMIC, gamax)
+    assert np.array_equal(gw.cpu().numpy().view(np.uint32), want_w.view(np.uint32)), "GPTQ block weights mismatch"
+    assert np.array_equal(ge.cpu().numpy().view(np.uint32), want_e.view(np.uint32)), "GPTQ block errors mismatch"
     torch.cuda.synchronize()
     print("smoke ok: collect / fake quant (NVFP4, FP8, INT8) / pack (NVFP4, INT4) / grouped and fused launches / histogram + "
-          "amax searches / MSE sweep / Hadamard rotation match the oracle")
+          "amax searches / MSE sweep / Hadamard rotation / GPTQ block match the oracle")
