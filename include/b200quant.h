@@ -396,6 +396,16 @@ int b200q_nvfp4_fp8_scale_sweep_ex(const void *w, int dtype, size_t n_blocks, co
 int b200q_nvfp4_fp8_scale_sweep_hessian(const void *w, int dtype, size_t cout, size_t n_cin_blocks,
                                         const float *cand_scales, const float *cand_amaxes, int n_cand,
                                         const float *hessian, float *best_amax, b200q_stream_t stream);
+/* Static NVFP4 per-block multiplier search (MseCalibrator on the blocked weight, calib/mse.py:84-172; the
+ * Four-Over-Six preset is mult = {1.0, 1.5} at fp8_max_norm 256): w is [n_blocks, 16]; for block b and candidate k,
+ * loss[k, b] = sum_e (x_e - fq(x_e; amax0[b] * mult[k]))^2 with x the fp32 widening of w and fq the static NVFP4 fake
+ * quant (as b200q_fake_quant_nvfp4_static with quantized block scales at fp8_max_norm) with an fp32 output; the
+ * difference and the square are each rounded, and the 16 squares are summed in the order of ATen's CUDA
+ * sum(dim=1).  best_amax[b] = amax0[b] * mult[k*] in fp32, k* = torch.argmin over k (first NaN, else first minimum).
+ * loss_out (nullable): [n_cand, n_blocks] fp32.  1 <= n_cand <= 128. */
+int b200q_nvfp4_static_mse_sweep(const void *w, int dtype, size_t n_blocks, const float *amax0,
+                                 const float *global_amax, const float *mult, int n_cand, float fp8_max_norm,
+                                 float *best_amax, float *loss_out, b200q_stream_t stream);
 
 /* ---- (4) input rotation (normalized Hadamard transform) --------------------------------- */
 

@@ -79,6 +79,7 @@ _SIGNATURES = {
     "b200q_nvfp4_fp8_scale_sweep": [_P, c_int, c_size_t, _P, _P, _P],
     "b200q_nvfp4_fp8_scale_sweep_ex": [_P, c_int, c_size_t, _P, _P, c_int, _P, _P],
     "b200q_nvfp4_fp8_scale_sweep_hessian": [_P, c_int, c_size_t, c_size_t, _P, _P, c_int, _P, _P, _P],
+    "b200q_nvfp4_static_mse_sweep": [_P, c_int, c_size_t, _P, _P, _P, c_int, c_float, _P, _P, _P],
     "b200q_hadamard": [_P, _P, c_int, c_size_t, c_size_t, c_size_t, _P, _P],
     "b200q_fake_quant_nvfp4_rotated": [_P, _P, c_int, c_size_t, c_size_t, c_size_t, c_int, _P, c_int, _P],
     "b200q_gptq_block": [_P, c_size_t, c_size_t, c_int, _P, c_size_t, _P, c_int, _P, c_int, c_size_t, c_size_t,

@@ -43,6 +43,7 @@ import torch
 
 from . import ops
 from .nn.functional import normalized_hadamard_transform
+from .nn.tensor_quantizer import fp8_max_for_normalization
 from .tensor_quant import dynamic_block_quant, fake_tensor_quant, scaled_e4m3, static_blockwise_fp4_fake_quant
 
 stats: collections.Counter = collections.Counter()
@@ -74,17 +75,11 @@ def b200_fake_quant_entrypoint(inputs: torch.Tensor, tq) -> torch.Tensor:
         return dynamic_block_quant(inputs, block, amax, None, num_bits, scale_bits, None, "dynamic", ptb)
     if getattr(tq, "_global_amax", None) is not None and num_bits == (2, 1):
         return static_blockwise_fp4_fake_quant(inputs, tq._amax.float(), tq._global_amax, True,
-                                               _fp8_max_for_normalization(tq), None, ptb)
+                                               fp8_max_for_normalization(tq), None, ptb)
     amax = _dynamic_amax(inputs, tq)
     if isinstance(num_bits, tuple):
         return scaled_e4m3(inputs, amax, None, num_bits[0], num_bits[1], None, ptb)
     return fake_tensor_quant(inputs, amax, None, num_bits, tq._unsigned, tq._narrow_range, None, ptb)
-
-
-def _fp8_max_for_normalization(tq) -> float:
-    """utils/numeric_utils.py:181-184: 256 for NVFP4 "four-over-six", else 448."""
-    bs = getattr(tq, "_block_sizes", None) or {}
-    return 256.0 if bs.get("four_over_six", False) else 448.0
 
 
 # ---- (4) extension-module shims (same names as tensor_quant.cpp:63-77 / tensor_quant_gpu_fp8.cu:109-114)
@@ -244,12 +239,14 @@ def _make_sweep_calibrator(base):
 
 def _make_mse_factory(base, ref_mse_cls):
     from .calib.mse import MseCalibrator as Mine
+    from .calib.mse import is_static_nvfp4_search
 
     class B200MseCalibrator(ref_mse_cls):
         """Stands in for ``MseCalibrator`` in model_calib.py:720-728 (a subclass, so the reference's
         ``isinstance(..., MseCalibrator)`` checks keep working).  For a quantizer on the b200 backend with an integer
-        or FP8 format the search runs as one fused sweep kernel; outside that scope (custom error function, no
-        quantizer behind ``quant_func``, other formats / backends) the host application's own methods run."""
+        or FP8 format, or static NVFP4 (16-element blocks, fp32 block amax, a global amax; Four-Over-Six included),
+        the search runs as one fused sweep kernel; outside that scope (custom error function, no quantizer behind
+        ``quant_func``, other formats / backends) the host application's own methods run."""
 
         def __init__(self, amax, axis=None, step_size=0.1, start_multiplier=0.25, stop_multiplier=4.0,
                      quant_func=None, error_func=None):
@@ -258,7 +255,8 @@ def _make_mse_factory(base, ref_mse_cls):
             q = getattr(quant_func, "keywords", {}).get("quantizer") if quant_func is not None else None
             nb = getattr(q, "_num_bits", None)
             ok = (error_func is None and q is not None and getattr(q, "backend", None) == "b200"
-                  and (isinstance(nb, int) or nb == (4, 3)) and not getattr(q, "is_mx_format", False)
+                  and ((isinstance(nb, int) or nb == (4, 3)) and not getattr(q, "is_mx_format", False)
+                       or is_static_nvfp4_search(q, amax))
                   and amax is not None and amax.is_cuda)
             self._b200 = Mine(amax, axis, step_size, start_multiplier, stop_multiplier, quant_func, None) if ok else None
 

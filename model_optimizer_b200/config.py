@@ -37,6 +37,11 @@ class RotateConfig:
         return dataclasses.replace(self, **(update or {}))
 
 
+# the non-integer keys block_sizes accepts (config.py:548,564); "four_over_six": static NVFP4 weights whose block
+# scales are normalized by 256 instead of 448 (Four-Over-Six, utils/numeric_utils.py:181-184)
+BLOCK_SIZES_STR_KEYS = ("type", "scale_bits", "scale_block_sizes", "four_over_six")
+
+
 @dataclass
 class QuantizerAttributeConfig:
     """quantization/config.py:322-709 (fields on the PTQ hot path only)."""
@@ -69,6 +74,12 @@ class QuantizerAttributeConfig:
             self.block_sizes = bs
             if self.axis is not None:
                 raise ValueError("axis and block_sizes are mutually exclusive")
+            for k, v in bs.items():                      # config.py:555-566
+                if isinstance(k, str):
+                    if k not in BLOCK_SIZES_STR_KEYS:
+                        raise ValueError(f"unknown block_sizes key {k!r}, expected one of {BLOCK_SIZES_STR_KEYS}")
+                elif not (isinstance(k, int) and (v is None or isinstance(v, int))):
+                    raise ValueError(f"block_sizes entry {k!r}: {v!r} must map an int axis to an int or None")
         if self.bias is not None:
             if self.bias.get("type", "static") not in ("static", "dynamic"):
                 raise ValueError(f"Invalid bias type: {self.bias['type']}, expected 'static' or 'dynamic'")
@@ -181,6 +192,12 @@ FP8_2D_BLOCKWISE_WEIGHT_ONLY_CFG = _preset(
 NVFP4_DEFAULT_CFG = _preset(_NVFP4, _NVFP4, "max")
 NVFP4_W4A4_WEIGHT_MSE_FP8_SWEEP_CFG = _preset(_NVFP4_STATIC, _NVFP4, {"method": "mse", "fp8_scale_sweep": True})
 NVFP4_W4A4_WEIGHT_LOCAL_HESSIAN_CFG = _preset(_NVFP4_STATIC, _NVFP4, {"method": "local_hessian", "fp8_scale_sweep": True})
+# Four-Over-Six (modelopt_recipes/configs/ptq/presets/model/nvfp4_four_over_six.yaml): static NVFP4 weights with
+# block scales normalized by 256; MSE over the multipliers {1.0, 1.5} picks, per 16-element block, the scale that
+# maps the block maximum to 6 or the one that maps it to 4
+NVFP4_FOUR_OVER_SIX_CFG = _preset({**_NVFP4_STATIC, "block_sizes": {**_NVFP4_STATIC["block_sizes"], "four_over_six": True}},
+                                  _NVFP4, {"method": "mse", "fp8_scale_sweep": False, "start_multiplier": 1.0,
+                                           "stop_multiplier": 1.5, "step_size": 0.5})
 NVFP4_AWQ_LITE_CFG = _preset(_NVFP4, _NVFP4, "awq_lite")
 NVFP4_AWQ_CLIP_CFG = _preset(_NVFP4, _NVFP4, {"method": "awq_clip"})
 W4A16_NVFP4_CFG = _preset_entries([("*weight_quantizer", _NVFP4)], "max")

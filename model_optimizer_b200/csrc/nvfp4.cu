@@ -365,16 +365,7 @@ __global__ void __launch_bounds__(kNvThreads)
     if (i >= n_blocks) continue;
     const uint32_t mb = b[u].prep_and_absmax_bits();
     const bool finite = mb < 0x7f800000u;
-    const float s = ss.block_scale(am[u]);
-    // nvfp4_scalar_quant (nvfp4_quant.py:87-100): zero scale -> zero block; nan/inf scale -> 1
-    const bool zero = (s == 0.0f);
-    const float s_safe = (zero || !(fabsf(s) <= 3.4028234664e38f)) ? 1.0f : s;
-    if (zero) {
-#pragma unroll
-      for (int w = 0; w < Block<Tag, VB>::WORDS; ++w) b[u].word(w) = 0u;
-    } else {
-      qdq_block<Tag, VB>(b[u], s_safe, finite && s_safe > 0.f);
-    }
+    static_qdq_block<Tag, VB>(b[u], ss.block_scale(am[u]), finite);
     b[u].store(y, i);
   }
 }

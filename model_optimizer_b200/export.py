@@ -12,6 +12,7 @@ from __future__ import annotations
 import torch
 
 from . import ops
+from .nn.tensor_quantizer import fp8_max_for_normalization
 from .qtensor import MXFP4QTensor, MXFP8QTensor, NVFP4QTensor
 
 QUANTIZATION_NONE = None
@@ -62,7 +63,8 @@ def get_quantization_format(module) -> str | None:
 
 
 def get_scaling_factor(quantizer):
-    """quant_utils.py:225-242: ``amax.float() / maxbound`` (NVFP4: global amax / (6 * 448))."""
+    """quant_utils.py:225-242: ``amax.float() / maxbound`` (NVFP4: global amax / (6 * 448), or / (6 * 256) for
+    Four-Over-Six, nvfp4_tensor.py:88-107)."""
     if quantizer is None or not quantizer.is_enabled:
         return None
     amax = quantizer.export_amax()
@@ -71,7 +73,7 @@ def get_scaling_factor(quantizer):
     if quantizer.num_bits == (2, 1):
         g = getattr(quantizer, "_global_amax", None)
         src = g if g is not None else quantizer._amax
-        sf = _tdiv(src.float(), 6.0 * 448.0)
+        sf = _tdiv(src.float(), 6.0 * fp8_max_for_normalization(quantizer))
     else:
         sf = _tdiv(amax.float(), quantizer.maxbound)
     assert torch.all(sf > 0), f"scaling factor {sf} not positive."
@@ -126,12 +128,14 @@ def pack_int4_in_uint8(weight, weights_scaling_factor):
 
 def export_nvfp4_weight(module):
     """(packed uint8 [N, K/2], e4m3 block scales [N, K/block], fp32 weight_scale_2): dynamic quantizers pack
-    from the calibrated per-tensor amax, static ones from their per-block amax (nvfp4_tensor.py:113-167)."""
+    from the calibrated per-tensor amax, static ones from their per-block amax (nvfp4_tensor.py:113-167), with the
+    block scales normalized by 256 instead of 448 for Four-Over-Six."""
     wq = module.weight_quantizer
     w = module.weight.detach().contiguous()
     bs = (wq.block_sizes or {}).get(-1, 16)
     if getattr(wq, "_global_amax", None) is not None:
-        return ops.pack_nvfp4(w, wq._global_amax.reshape(1).float(), wq._amax.float().reshape(-1), block_size=bs)
+        return ops.pack_nvfp4(w, wq._global_amax.reshape(1).float(), wq._amax.float().reshape(-1),
+                              fp8_max_norm=fp8_max_for_normalization(wq), block_size=bs)
     return ops.pack_nvfp4(w, wq._amax.reshape(1).float(), block_size=bs)
 
 

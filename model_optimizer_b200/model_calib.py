@@ -177,9 +177,10 @@ def mse_calibrate(model: nn.Module, forward_loop: Callable | None = None, distri
     ``fp8_scale_sweep=True``: only static NVFP4 weights, per-block argmin over the 126 FP8-E4M3 scale values
     (``NVFP4MSECalibrator``, calib/mse.py:175-311) -- one ``b200q_nvfp4_fp8_scale_sweep`` launch per weight.
     Otherwise: the multiplier search of ``MseCalibrator`` (calib/mse.py:31-172) for every enabled, static,
-    non-MX weight quantizer -- one ``b200q_mse_sweep[_rows]`` launch per weight (the reference: 39 x ~4 passes)."""
-    from .calib.mse import MseCalibrator
-
+    non-MX weight quantizer -- one ``b200q_mse_sweep[_rows]`` launch per weight (the reference: 39 x ~4 passes), or
+    for static NVFP4 weights one ``b200q_nvfp4_static_mse_sweep`` launch that picks each 16-element block's
+    multiplier against the ``global_amax`` set by max calibration (shared by q/k/v and gate/up siblings).  With the
+    Four-Over-Six preset's multipliers {1.0, 1.5} this chooses, per block, the grid that ends at 6 or at 4."""
     max_calibrate(model, forward_loop, distributed_sync)
     for m in model.modules():
         if not is_quantized_linear(m):
@@ -191,22 +192,30 @@ def mse_calibrate(model: nn.Module, forward_loop: Callable | None = None, distri
         if fp8_scale_sweep:
             if not q.is_nvfp4_static:
                 continue                                     # left at the max-calibrated amax (:717-718)
+            # the sweep's candidates and losses do not depend on the FP8 normalization: a Four-Over-Six quantizer is
+            # swept like any static NVFP4 one (NVFP4MSECalibrator, calib/mse.py:175-311) and normalizes by 256 after
             best = ops.nvfp4_fp8_scale_sweep(m.weight.contiguous(), q._global_amax.reshape(1))
             q.amax = best.reshape(q._amax.shape)
             continue
-        if q.is_nvfp4_static:
-            raise NotImplementedError("mse_calibrate: static NVFP4 weights are searched with fp8_scale_sweep=True")
-        from functools import partial
+        _mse_search_weight(m, step_size, start_multiplier, stop_multiplier)
 
-        cal = MseCalibrator(q._amax.clone().detach(), q._calibrator._axis, step_size, start_multiplier,
-                            stop_multiplier, quant_func=partial(_mse_quant_func, quantizer=q))
-        w = m.weight
-        if q.is_static_block_quant:                          # the calibration layout: [n_blocks, block]
-            q._setup_for_blockquant(w)
-            w = q._process_for_blockquant(w)
-        cal.collect(w)
-        q.amax = cal.compute_amax()
-        cal.reset()
+
+def _mse_search_weight(m, step_size, start_multiplier, stop_multiplier):
+    """The multiplier search of one weight (``_make_weight_mse_calibrator`` -> ``MseCalibrator``, :720-728)."""
+    from functools import partial
+
+    from .calib.mse import MseCalibrator
+
+    q = m.weight_quantizer
+    cal = MseCalibrator(q._amax.clone().detach(), q._calibrator._axis, step_size, start_multiplier,
+                        stop_multiplier, quant_func=partial(_mse_quant_func, quantizer=q))
+    w = m.weight
+    if q.is_static_block_quant:                              # the calibration layout: [n_blocks, block]
+        q._setup_for_blockquant(w)
+        w = q._process_for_blockquant(w)
+    cal.collect(w)
+    q.amax = cal.compute_amax()
+    cal.reset()
 
 
 @torch.no_grad()
@@ -258,10 +267,13 @@ def local_hessian_calibrate(model: nn.Module, forward_loop: Callable | None = No
         if q._dynamic or q.is_mx_format or getattr(q, "_amax", None) is None:
             continue
         e = acc.get(id(q))
+        hess = None if e is None or e[1] == 0 else e[0] / e[1]
         if fp8_scale_sweep and q.is_nvfp4_static:
-            hess = None if e is None or e[1] == 0 else e[0] / e[1]
             best = ops.nvfp4_fp8_scale_sweep(m.weight.contiguous(), q._global_amax.reshape(1), hessian=hess)
             q.amax = best.reshape(q._amax.shape)
+        elif not fp8_scale_sweep and hess is None and q._calibrator is not None:
+            # no Hessian for this weight: the reference's plain squared-error multiplier search (:1085-1095)
+            _mse_search_weight(m, step_size, start_multiplier, stop_multiplier)
     if debug:
         model._local_hessian_accumulators = acc
 

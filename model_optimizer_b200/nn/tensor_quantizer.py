@@ -36,6 +36,14 @@ def _qtensor_base():
     return _QT_BASE
 
 
+def fp8_max_for_normalization(quantizer) -> float:
+    """The FP8 maximum that normalizes static NVFP4 block scales (utils/numeric_utils.py:181-184): 256 for
+    Four-Over-Six (``block_sizes["four_over_six"]`` truthy), else 448.  The fake quant, the real quant, the export
+    and the drop-in all take it from here."""
+    bs = getattr(quantizer, "block_sizes", None) or {}
+    return 256.0 if bool(bs.get("four_over_six", False)) else 448.0
+
+
 class TensorQuantizer(nn.Module):
     # input quantizers of sibling linears that are handed the very same tensor object (q/k/v, gate/up) do the collect /
     # fake quant once (nn/shared_input.py); bit-identical results
@@ -523,8 +531,8 @@ class TensorQuantizer(nn.Module):
                                        bs.get("scale_bits"), None, "dynamic", self._pass_through_bwd)
         if self.is_nvfp4_static:  # StaticBlockScaleQuantizer._fake_quantize (:1708-1731)
             gamax = getattr(self, "_global_amax", None)
-            return static_blockwise_fp4_fake_quant(inputs, self._get_amax(inputs).float(), gamax, True, 448.0,
-                                                   None, self._pass_through_bwd)
+            return static_blockwise_fp4_fake_quant(inputs, self._get_amax(inputs).float(), gamax, True,
+                                                   fp8_max_for_normalization(self), None, self._pass_through_bwd)
         amax = self._get_amax(inputs)
         if isinstance(self._num_bits, tuple):
             e, m = self._num_bits
@@ -550,12 +558,17 @@ class TensorQuantizer(nn.Module):
                                  "Expected (2, 1) for MXFP4 or (4, 3) for MXFP8.")
             self._scale = sc
         elif self._num_bits == (2, 1):
+            if bs and bs.get("four_over_six", False):   # tensor_quantizer.py:861-866
+                raise NotImplementedError(
+                    "NVFP4 Four-Over-Six (4/6) is not supported via mtq.compress: the per-block M=4/M=6 choice baked "
+                    "into the quantizer amax by MSE calibration is not preserved by real quantization. Use "
+                    "mtq.quantize + export for 4/6 instead.")
             # second-level scale from the calibration when there is one (tensor_quantizer.py:867-875,
             # NVFP4QTensor.get_weights_scaling_factor_2_from_quantizer): the static global amax, else _amax
             wsf2 = None
             if self.amax is not None:
                 g = getattr(self, "_global_amax", None) if self.is_static_block_quant else None
-                wsf2 = (g if g is not None else self._amax).float() / (6.0 * 448.0)
+                wsf2 = (g if g is not None else self._amax).float() / (6.0 * fp8_max_for_normalization(self))
             q, sf, sf2 = NVFP4QTensor.quantize(inputs, bs[-1], weights_scaling_factor_2=wsf2)
             self._scale, self._double_scale = sf, sf2
         elif bs and bs.get("scale_bits", 0) == 8 and bs.get("scale_block_sizes"):
@@ -676,4 +689,4 @@ class TensorQuantizer(nn.Module):
                 f"amax={amax} calib={self._if_calib} quant={self._if_quant}" + self._rotate_repr())
 
 
-__all__ = ["TensorQuantizer"]
+__all__ = ["TensorQuantizer", "fp8_max_for_normalization"]

@@ -901,6 +901,34 @@ def nvfp4_fp8_scale_sweep(w, global_amax, candidates="device", hessian=None):
     return best
 
 
+def nvfp4_static_mse_sweep(w, amax0, global_amax, mult, fp8_max_norm=448.0, loss_out=None):
+    """Static NVFP4 per-block multiplier search (``MseCalibrator`` on the blocked weight, calib/mse.py:84-172) ->
+    fp32 ``best_amax`` [n_blocks] = ``amax0 * mult[argmin_k loss[k]]``, one launch.  ``w``: the weight, 16 elements
+    per block (bf16, fp16 or fp32); ``amax0``: the fp32 per-block amax; ``mult``: at most 128 fp32 multipliers
+    (``torch.linspace(start, stop, steps)`` on the weight's device, as the calibrator builds them); ``fp8_max_norm``:
+    256 for Four-Over-Six, else 448.  ``loss_out``: an optional fp32 [n_cand, n_blocks] tensor that receives
+    every block's loss per candidate."""
+    w = _prep(w, "w")
+    n_blocks = w.numel() // 16
+    if n_blocks * 16 != w.numel():
+        raise B200QuantError("w.numel() must be a multiple of 16")
+    if amax0.numel() != n_blocks:
+        raise B200QuantError(f"amax0 has {amax0.numel()} values for {n_blocks} blocks")
+    a0 = amax0.detach().to(device=w.device, dtype=torch.float32).contiguous()
+    g = global_amax.detach().to(device=w.device, dtype=torch.float32).reshape(-1).contiguous()
+    if g.numel() != 1:
+        raise B200QuantError("global_amax must hold one value")
+    mult = mult.detach().to(device=w.device, dtype=torch.float32).contiguous()
+    if loss_out is not None and (loss_out.dtype != torch.float32 or not loss_out.is_cuda
+                                 or not loss_out.is_contiguous() or loss_out.numel() != mult.numel() * n_blocks):
+        raise B200QuantError("loss_out must be a contiguous float32 CUDA tensor of n_cand * n_blocks elements")
+    best = torch.empty(n_blocks, dtype=torch.float32, device=w.device)
+    call("b200q_nvfp4_static_mse_sweep", w.data_ptr(), _dt(w), n_blocks, a0.data_ptr(), g.data_ptr(),
+         mult.data_ptr(), mult.numel(), float(fp8_max_norm), best.data_ptr(),
+         None if loss_out is None else loss_out.data_ptr(), _stream(w))
+    return best
+
+
 # ------------------------------------------------------------------------------------------------
 # GPTQ weight calibration
 # ------------------------------------------------------------------------------------------------

@@ -119,6 +119,15 @@ def run():
     ge = ops.gptq_block_update(gw, gu, ops.GPTQ_NVFP4_DYNAMIC, gamax)
     assert np.array_equal(gw.cpu().numpy().view(np.uint32), want_w.view(np.uint32)), "GPTQ block weights mismatch"
     assert np.array_equal(ge.cpu().numpy().view(np.uint32), want_e.view(np.uint32)), "GPTQ block errors mismatch"
+    # (8) the Four-Over-Six block search (static NVFP4 at 256, multipliers {1.0, 1.5}) against the oracle
+    from tools import nvfp4_mse_oracle
+
+    fa0 = o.round_bf16(np.abs(xh).reshape(-1, 16).max(axis=1))
+    fg = np.float32(fa0.max())
+    fmult = torch.linspace(1.0, 1.5, 2, device="cuda")
+    fbest = ops.nvfp4_static_mse_sweep(x, torch.from_numpy(fa0).cuda(), torch.tensor([fg], device="cuda"), fmult, 256.0)
+    fwant, _, _ = nvfp4_mse_oracle.search(xh, fa0, fg, fmult.cpu().numpy(), 256.0, "cuda")
+    assert np.array_equal(fbest.cpu().numpy().view(np.uint32), fwant.view(np.uint32)), "Four-Over-Six search mismatch"
     torch.cuda.synchronize()
     print("smoke ok: collect / fake quant (NVFP4, FP8, INT8) / pack (NVFP4, INT4) / grouped and fused launches / histogram + "
-          "amax searches / MSE sweep / Hadamard rotation / GPTQ block match the oracle")
+          "amax searches / MSE sweep / Hadamard rotation / GPTQ block / Four-Over-Six search match the oracle")
