@@ -50,6 +50,8 @@ int b200q_device_info(int *sm_count, int *cc_major, int *cc_minor);
 int b200q_set_device(int device);
 /* Launch-shape tuning knob (bench / autotune only).  key: "amax_unroll", "ew_unroll", "vec_bytes". */
 int b200q_set_tuning(const char *key, int value);
+/* The value a knob holds (0: unset, the built-in default applies). */
+int b200q_get_tuning(const char *key, int *value);
 
 /* ---- (1) calibration collect ------------------------------------------------------------ */
 

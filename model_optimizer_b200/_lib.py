@@ -29,6 +29,7 @@ _P = c_void_p
 _SIGNATURES = {
     "b200q_device_info": [_P, _P, _P],
     "b200q_set_tuning": [c_char_p, c_int],
+    "b200q_get_tuning": [c_char_p, _P],
     "b200q_set_device": [c_int],
     "b200q_amax_per_tensor": [_P, c_int, c_size_t, _P, _P],
     "b200q_amax_rows": [_P, c_int, c_size_t, c_size_t, c_size_t, _P, _P],
@@ -129,6 +130,12 @@ def set_tuning(key: str, value: int) -> None:
     call("b200q_set_tuning", key.encode(), int(value))
 
 
+def get_tuning(key: str) -> int:
+    v = c_int(0)
+    call("b200q_get_tuning", key.encode(), ctypes.byref(v))
+    return v.value
+
+
 def device_info() -> tuple[int, int, int]:
     sm, ma, mi = c_int(0), c_int(0), c_int(0)
     call("b200q_device_info", ctypes.byref(sm), ctypes.byref(ma), ctypes.byref(mi))
@@ -144,6 +151,7 @@ __all__ = [
     "LIB_PATH",
     "call",
     "device_info",
+    "get_tuning",
     "load",
     "set_tuning",
     "c_double",

@@ -99,10 +99,16 @@ __global__ void __launch_bounds__(kGptqThreads) gptq_block_kernel(GptqArgs a) {
         const int i = i0 + k;
         if (i >= nb) break;  // warp-uniform
         uint32_t mb = 0;     // |w| max of the 16-element block, as fp32 bits (NaN-propagating)
+        uint32_t mn = 0;     // 1 + the bits of the NaN-ignoring |w| max (dyn_block_max); 0: every element is NaN
         if constexpr (FMT == kGptqNvfp4Static || FMT == kGptqNvfp4Dyn) {
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) mb = max(mb, __float_as_uint(w[kk]) & 0x7fffffffu);
+          for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t a = __float_as_uint(w[kk]) & 0x7fffffffu;
+            mb = max(mb, a);
+            mn = max(mn, a <= 0x7f800000u ? a + 1u : 0u);
+          }
           mb = group_max<4>(mb);
+          if constexpr (FMT == kGptqNvfp4Dyn) mn = group_max<4>(mn);
         }
         float err = 0.f;
         if (lane == owner) {
@@ -118,7 +124,7 @@ __global__ void __launch_bounds__(kGptqThreads) gptq_block_kernel(GptqArgs a) {
             const bool fast = mb < 0x7f800000u && s_st > 0.f && s_st >= 0x1p-40f && s_st <= 0x1p60f;
             q = zero_st ? 0.f : qdq_e2m1_one(__fadd_rn(x, 0.f), s_st, dst, fast);
           } else {
-            const float s = ds.block_scale(__uint_as_float(mb), d6);
+            const float s = ds.block_scale(mn ? __uint_as_float(mn - 1u) : __uint_as_float(0x7fc00000u), d6);
             const bool fast = mb < 0x7f800000u && s >= 0x1p-40f && s <= 0x1p60f;
             q = qdq_e2m1_one(__fadd_rn(x, 0.f), s, ExactDiv(s), fast);
           }

@@ -190,7 +190,7 @@ __global__ void __launch_bounds__(SMEM ? kHadMaxThreads : kHadThreads)
 #pragma unroll
     for (int v = 0; v < VPT; ++v) {
       const uint32_t mb = b[v].prep_and_absmax_bits();
-      qdq_block<Tag, 32>(b[v], ds.block_scale(__uint_as_float(mb), d6), mb < 0x7f800000u);
+      qdq_block<Tag, 32>(b[v], ds.block_scale(dyn_block_max(b[v], mb), d6), mb < 0x7f800000u);
     }
     if constexpr (MODE == 2) {
 #pragma unroll

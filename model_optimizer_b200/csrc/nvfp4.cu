@@ -44,7 +44,7 @@ __global__ void __launch_bounds__(kNvThreads)
     if (i >= n_blocks) continue;
     const uint32_t mb = b[u].prep_and_absmax_bits();
     const bool finite = mb < 0x7f800000u;
-    const float s = ds.block_scale(__uint_as_float(mb), d6);
+    const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
     qdq_block<Tag, VB>(b[u], s, finite);
     b[u].store(y, i);
   }
@@ -74,7 +74,7 @@ __global__ void __launch_bounds__(kNvThreads)
   for (int u = 0; u < UNROLL; ++u) {
     const uint32_t mb = b[u].prep_and_absmax_bits();
     const bool finite = mb < 0x7f800000u;
-    const float s = ds.block_scale(__uint_as_float(mb), d6);
+    const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
     qdq_block<Tag, VB>(b[u], s, finite);
     Vec<VB> *sp = reinterpret_cast<Vec<VB> *>(s_out) + ((size_t)u * kNvThreads + threadIdx.x) * Block<Tag, VB>::NV;
 #pragma unroll
@@ -118,7 +118,7 @@ __device__ __forceinline__ uint32_t dyn_fq_blocks(const uint8_t *__restrict__ x,
       mb = b[u].prep_and_absmax_bits();
     }
     const bool finite = mb < 0x7f800000u;
-    const float s = ds.block_scale(__uint_as_float(mb), d6);
+    const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
     qdq_block<Tag, VB>(b[u], s, finite);
     b[u].store(y, i);
   }
@@ -274,15 +274,11 @@ __global__ void __launch_bounds__(kNvThreads)
     const size_t c0 = bk * kBlk;
     const int cnt = (int)((row_len - c0) < (size_t)kBlk ? (row_len - c0) : (size_t)kBlk);
     float f[kBlk];
-    float bmax = 0.f;
-    bool finite = true;
+    float bmax = __uint_as_float(0x7fc00000u);   // NaN-ignoring max, as dyn_block_max
     for (int e = 0; e < kBlk; ++e) {
       f[e] = e < cnt ? Elem<Tag>::load1(x, row * row_len + c0 + e) : 0.0f;
-      const float a = fabsf(f[e]);
-      if (!(a <= 3.4028234664e38f)) finite = false;
-      bmax = fmaxf(bmax, a);
+      bmax = fmaxf(bmax, fabsf(f[e]));
     }
-    if (!finite) bmax = __uint_as_float(0x7fc00000u);
     const float s = ds.block_scale(bmax, d6);
     for (int e = 0; e < cnt; ++e) {
       const float r = __fmul_rn(e2m1_round_mag(__fdiv_rn(fabsf(f[e]), s)), s);

@@ -150,6 +150,17 @@ int b200q_set_tuning(const char *key, int value) {
   return B200Q_ERR_INVALID;
 }
 
+int b200q_get_tuning(const char *key, int *value) {
+  if (!key || !value) return B200Q_ERR_INVALID;
+  for (auto &k : g_knobs)
+    if (strcmp(k.key, key) == 0) {
+      *value = k.value;
+      return B200Q_OK;
+    }
+  set_error("unknown tuning key '%s'", key);
+  return B200Q_ERR_INVALID;
+}
+
 int b200q_selftest_fastdiv(uint64_t seed, size_t n, unsigned long long *mismatches_host) {
   B200Q_REQUIRE(mismatches_host != nullptr, "mismatches_host is null");
   unsigned long long *d = nullptr;

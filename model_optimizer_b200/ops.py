@@ -455,11 +455,21 @@ def _amax_arg(amax: torch.Tensor, like: torch.Tensor) -> torch.Tensor:
     return amax if amax.is_contiguous() else amax.contiguous()
 
 
+def _out_arg(out, x: torch.Tensor) -> torch.Tensor:
+    """``out`` (or a new tensor like ``x`` when None), refused unless the kernel can write all of x's elements to it."""
+    if out is None:
+        return torch.empty_like(x)
+    if not isinstance(out, torch.Tensor) or out.device != x.device or out.dtype != x.dtype or out.shape != x.shape \
+            or not out.is_contiguous():
+        raise B200QuantError(f"out must be a contiguous {x.dtype} tensor of shape {tuple(x.shape)} on {x.device}")
+    return out
+
+
 def fake_quant_int(x, amax, num_bits=8, unsigned=False, narrow_range=True, outer=1, out=None):
     """Integer fake quant; ``amax[(i // outer) % amax.numel()]`` scales element i."""
     x = _prep(x, "x")
     amax = _amax_arg(amax, x)
-    y = torch.empty_like(x) if out is None else out
+    y = _out_arg(out, x)
     call("b200q_fake_quant_int", x.data_ptr(), y.data_ptr(), _dt(x), x.numel(), amax.data_ptr(), _dt(amax),
          amax.numel(), int(outer), int(num_bits), int(bool(unsigned)), int(bool(narrow_range)), _stream(x))
     return y
@@ -469,7 +479,7 @@ def fake_quant_fp8(x, amax=None, outer=1, out=None, eager=False):
     """FP8-E4M3 fake quant (amax=None: plain torch-style cast round trip).  ``eager``: the scale rule of the
     reference's _fp8_eager (reciprocal * 448) instead of the CUDA extension's 448 / amax."""
     x = _prep(x, "x")
-    y = torch.empty_like(x) if out is None else out
+    y = _out_arg(out, x)
     if amax is None:
         call("b200q_fake_quant_fp8", x.data_ptr(), y.data_ptr(), _dt(x), x.numel(), None, 0, 1, 1, _stream(x))
         return y
@@ -483,7 +493,7 @@ def fake_quant_nvfp4(x, global_amax, out=None):
     """NVFP4 dynamic block-16 fake quant along the last dim."""
     x = _prep(x, "x")
     global_amax = _amax_arg(global_amax, x)
-    y = torch.empty_like(x) if out is None else out
+    y = _out_arg(out, x)
     row_len = x.shape[-1] if x.dim() > 0 else 1
     n_rows = x.numel() // row_len if row_len else 0
     call("b200q_fake_quant_nvfp4", x.data_ptr(), y.data_ptr(), _dt(x), n_rows, row_len,
@@ -548,7 +558,7 @@ def fake_quant_nvfp4_static(x, block_amax, global_amax=None, quantize_block_scal
     if global_amax is not None:
         global_amax = global_amax.to(device=x.device, dtype=torch.float32).contiguous()
         gptr = global_amax.data_ptr()
-    y = torch.empty_like(x) if out is None else out
+    y = _out_arg(out, x)
     call("b200q_fake_quant_nvfp4_static", x.data_ptr(), y.data_ptr(), _dt(x), n_blocks, 16,
          block_amax.data_ptr(), gptr, int(bool(quantize_block_scales)), float(fp8_max_norm), _stream(x))
     return y
@@ -722,7 +732,7 @@ def fake_quant_mx(x, block_size, elem_format, out=None):
     """fused_amax_convert(x, block_size, elem_format, E8M0): blocks along the last dim."""
     x = _prep(x, "x")
     fmt = MX_FORMATS[elem_format] if isinstance(elem_format, str) else int(elem_format)
-    y = torch.empty_like(x) if out is None else out
+    y = _out_arg(out, x)
     k = x.shape[-1] if x.dim() else 1
     call("b200q_fake_quant_mx", x.data_ptr(), y.data_ptr(), _dt(x), x.numel() // max(k, 1), k, int(block_size), fmt,
          _stream(x))
@@ -793,7 +803,7 @@ def scale_cols(x, scale, out=None):
     x = _prep(x, "x")
     scale = _amax_arg(scale, x)
     c = scale.numel()
-    y = torch.empty_like(x) if out is None else out
+    y = _out_arg(out, x)
     call("b200q_scale_cols", x.data_ptr(), y.data_ptr(), _dt(x), x.numel() // c, c, scale.data_ptr(),
          _dt(scale), _stream(x))
     return y
@@ -803,7 +813,7 @@ def awq_scale_fake_quant(w, col_scale, block_size, num_bits=4, narrow_range=Fals
     w = _prep(w, "w")
     col_scale = _amax_arg(col_scale, w)
     c = w.shape[-1]
-    y = torch.empty_like(w) if out is None else out
+    y = _out_arg(out, w)
     call("b200q_awq_scale_fake_quant", w.data_ptr(), y.data_ptr(), _dt(w), w.numel() // c, c,
          col_scale.data_ptr(), _dt(col_scale), int(block_size), int(num_bits), int(bool(narrow_range)), _stream(w))
     return y

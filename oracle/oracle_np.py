@@ -331,7 +331,7 @@ def nvfp4_block_scale_dynamic(bmax, global_amax):
     gs_safe = gs if gs > 0 else F32(1e-12)
     with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
         sc = (np.asarray(bmax, dtype=F32) / F32(F32(6.0) * gs_safe)).astype(F32)
-        sc = np.minimum(sc, F32(448.0))
+        sc = np.fmin(sc, F32(448.0))                      # tl.minimum: NaN-ignoring (FMNMX)
         s = (e4m3_round(sc) * gs_safe).astype(F32)
     return np.where(s >= F32(1e-5), s, F32(1.0)).astype(F32)
 
@@ -354,7 +354,8 @@ def fake_quant_nvfp4(x, global_amax, dtype="bf16"):
     if pad:
         x2 = np.concatenate([x2, np.zeros((x2.shape[0], pad), dtype=F32)], axis=1)
     xb = x2.reshape(x2.shape[0], -1, 16)
-    bmax = np.max(np.abs(xb), axis=2, keepdims=True)
+    with np.errstate(invalid="ignore"):                 # tl.max: NaN elements are skipped, an all-NaN block gives NaN
+        bmax = np.fmax.reduce(np.abs(xb), axis=2, keepdims=True)
     s = nvfp4_block_scale_dynamic(bmax, global_amax)
     out = _nvfp4_qdq_with_scale(xb, s).reshape(x2.shape)[:, :k]
     return round_to(out.reshape(shape), dtype)
@@ -656,7 +657,9 @@ def nvfp4_block_log2_hist(x, num_bins=512, log2_min=-40.0, log2_max=40.0):
     b = reduce_block_amax(x, 16).ravel()
     nz = b[b > 0]
     frac = ((np.log2(nz).astype(F32) - F32(log2_min)) / F32(log2_max - log2_min)).astype(F32)
-    idx = np.clip(np.floor((frac * F32(num_bins)).astype(F32)).astype(np.int64), 0, num_bins - 1)
+    # clamp before the integer conversion: +inf (an inf block) lands in the top bin, as CUDA's saturating float -> int64
+    # conversion and the kernel put it
+    idx = np.clip(np.floor((frac * F32(num_bins)).astype(F32)), 0, num_bins - 1).astype(np.int64)
     return np.bincount(idx, minlength=num_bins).astype(np.int64), (b.max() if b.size else F32(0))
 
 
