@@ -15,6 +15,7 @@ B200-first differences (results identical, work removed):
 from __future__ import annotations
 
 import collections
+import math
 import warnings
 from typing import Callable
 
@@ -227,8 +228,10 @@ def local_hessian_calibrate(model: nn.Module, forward_loop: Callable | None = No
     forward pre-hooks while the weight quantizers are disabled.  Static NVFP4 weights: ONE
     ``b200q_nvfp4_fp8_scale_sweep_hessian`` launch per weight (the reference: a Triton kernel with ``tl.dot``, or 126
     einsum passes); the Hessian itself is a batched GEMM (cuBLAS through ``torch.matmul`` -- a plain library GEMM,
-    not part of this engine).  Other weights (and ``cin % block_size != 0``) fall back to plain ``mse_calibrate``
-    semantics like the reference."""
+    not part of this engine).  ``fp8_scale_sweep=False``: every eligible static weight (not dynamic, not MX, with an
+    ``_amax``) gets the multiplier search, under the Hessian metric where it has a Hessian
+    (``_hessian_mse_search_weight``) and under the squared error where it has none (never reached by the forward, or
+    ``cin % block_size != 0``), like the reference."""
     if forward_loop is None:
         warnings.warn("forward_loop must be provided for local_hessian; skipping local_hessian")
         return
@@ -241,15 +244,10 @@ def local_hessian_calibrate(model: nn.Module, forward_loop: Callable | None = No
     def hook(lin, args):
         if not args:
             return
-        x = args[0]
         cin = lin.weight.shape[1]
         if cin % block_size:
             return
-        xt = x.reshape(-1, cin).to(torch.float32).T.reshape(cin // block_size, block_size, -1)
-        h = xt @ xt.transpose(-1, -2)
-        e = acc.setdefault(id(lin.weight_quantizer), [None, 0])
-        e[0] = h if e[0] is None else e[0].add_(h)
-        e[1] += x.numel() // cin
+        _local_hessian_update(acc.setdefault(id(lin.weight_quantizer), [None, 0]), args[0], cin, block_size)
 
     mods = [m for m in model.modules() if is_quantized_linear(m) and m.weight_quantizer.is_enabled]
     for m in mods:
@@ -271,11 +269,65 @@ def local_hessian_calibrate(model: nn.Module, forward_loop: Callable | None = No
         if fp8_scale_sweep and q.is_nvfp4_static:
             best = ops.nvfp4_fp8_scale_sweep(m.weight.contiguous(), q._global_amax.reshape(1), hessian=hess)
             q.amax = best.reshape(q._amax.shape)
-        elif not fp8_scale_sweep and hess is None and q._calibrator is not None:
-            # no Hessian for this weight: the reference's plain squared-error multiplier search (:1085-1095)
-            _mse_search_weight(m, step_size, start_multiplier, stop_multiplier)
+        elif not fp8_scale_sweep and q._calibrator is not None:
+            # the multiplier search (:720-728): under the Hessian metric where the forward reached this weight, else
+            # the plain squared error
+            if hess is None:
+                _mse_search_weight(m, step_size, start_multiplier, stop_multiplier)
+            else:
+                _hessian_mse_search_weight(m, hess, step_size, start_multiplier, stop_multiplier)
     if debug:
         model._local_hessian_accumulators = acc
+
+
+def _local_hessian_update(entry: list, x: torch.Tensor, cin: int, block_size: int = 16) -> list:
+    """``_LocalHessianAccumulator.accumulate`` (model_calib.py:848-860) on ``entry = [H, n_tokens]``: add the
+    per-cin-block ``X^T X`` of the activation ``x`` (``[..., cin]``, taken in fp32) to ``H`` ([cin / block_size,
+    block_size, block_size]; ``None`` before the first batch) and its token count to ``n_tokens``.  The normalized
+    Hessian is ``H / n_tokens``."""
+    xt = x.reshape(-1, cin).to(torch.float32).T.reshape(cin // block_size, block_size, -1)
+    h = xt @ xt.transpose(-1, -2)
+    entry[0] = h if entry[0] is None else entry[0].add_(h)
+    entry[1] += x.numel() // cin
+    return entry
+
+
+def _hessian_mse_search_weight(m, hess, step_size, start_multiplier, stop_multiplier, round_mult=True):
+    """``MseCalibrator`` with the local-Hessian ``error_func`` (calib/mse.py:84-172, model_calib.py:891-896) on one
+    weight: for every multiplier ``c`` of ``linspace(start, stop, ceil((stop - start) / step) + 1)``, fake-quantize the
+    fp32 weight at ``initial_amax * c`` with the quantizer itself, weight each element's error by the loss
+    ``dw^T H dw`` of its 16-element cin block (einsum ``cnb,nbd,cnd->cn``), sum that per amax slot, and keep the
+    ``torch.argmin`` multiplier.  ``round_mult``: the candidate amax as torch forms it on CUDA (the multiplier rounded
+    to the amax dtype first, ``MseCalibrator``'s default) or, False, on CPU.  A composed loop of torch and the engine's
+    fake-quant kernels (calibration only, off the hot path)."""
+    q = m.weight_quantizer
+    a0 = q._amax.clone().detach()
+    w = m.weight
+    if q.is_static_block_quant:                              # the calibration layout: [n_blocks, block]
+        q._setup_for_blockquant(w)
+        w = q._process_for_blockquant(w)
+    x = w.detach().to(torch.float32)
+    cout, bs = m.weight.shape[0], hess.shape[-1]
+    hess = hess.to(device=x.device, dtype=torch.float32)
+    axis = q._calibrator._axis                               # convert_quantization_axis_to_reduce_axis (:128-143)
+    if axis is not None:
+        keep = {a % x.dim() for a in ((axis,) if isinstance(axis, int) else axis)}
+        dims = [d for d in range(x.dim()) if d not in keep]
+    n_steps = math.ceil((stop_multiplier - start_multiplier) / step_size) + 1
+    cands = torch.linspace(start_multiplier, stop_multiplier, steps=n_steps, device=x.device)
+    losses = []
+    for c in cands:
+        amax = a0 * c
+        if not round_mult:
+            amax = (a0.float() * c).to(amax.dtype)
+        dw = (x - _mse_quant_func(x, amax, q)).view(cout, -1, bs)
+        block_loss = torch.einsum("cnb,nbd,cnd->cn", dw, hess, dw).reshape(-1)
+        err = block_loss.unsqueeze(-1).expand(-1, bs).reshape(x.shape)
+        losses.append(err.sum() if axis is None else err.sum(dim=dims) if dims else err)
+    best = cands[torch.argmin(torch.stack(losses), dim=0)]
+    if best.ndim:
+        best = best.view_as(a0)
+    q.amax = a0 * best
 
 
 def _mse_quant_func(x, amax, quantizer):

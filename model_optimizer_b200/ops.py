@@ -901,14 +901,21 @@ def nvfp4_fp8_scale_sweep(w, global_amax, candidates="device", hessian=None):
         raise B200QuantError(f"n_blocks ({n_blocks}) is not divisible by n_cin_blocks ({n_cin})")
     if cand is None:
         cand = fp8_scale_candidates("cpu").to(w.device)
-    g = global_amax.reshape(())
-    cand_amaxes = (cand * g).contiguous()                                      # nvfp4_fp8_sweep.py:268
-    # compute_fp4_scales(cand_amaxes, g, True) (fp4_kernel.py:215-249): amax / 6 through the FP8 fake quant
-    cand_scales = fake_quant_fp8((cand_amaxes / 6.0).contiguous(), (g * (448.0 / 448.0) / 6.0).reshape(1))
+    cand_scales, cand_amaxes = hessian_sweep_candidates(global_amax, cand)
     h = hessian.detach().to(device=w.device, dtype=torch.float32).contiguous()
     call("b200q_nvfp4_fp8_scale_sweep_hessian", w.data_ptr(), _dt(w), n_blocks // n_cin, n_cin, cand_scales.data_ptr(),
          cand_amaxes.data_ptr(), cand.numel(), h.data_ptr(), best.data_ptr(), _stream(w))
     return best
+
+
+def hessian_sweep_candidates(global_amax, cand):
+    """``(cand_scales, cand_amaxes)`` of the Hessian-weighted sweep (nvfp4_fp8_sweep.py:272-275), fp32 on ``cand``'s
+    device: ``cand_amaxes = cand * g`` and ``cand_scales = compute_fp4_scales(cand_amaxes, g, True)`` (fp4_kernel.py:
+    217-251), i.e. ``cand_amaxes / 6`` through the FP8 fake quant at amax ``g / 6``."""
+    g = global_amax.detach().to(device=cand.device, dtype=torch.float32).reshape(())
+    cand_amaxes = (cand * g).contiguous()
+    cand_scales = fake_quant_fp8((cand_amaxes / 6.0).contiguous(), (g * (448.0 / 448.0) / 6.0).reshape(1))
+    return cand_scales, cand_amaxes
 
 
 def nvfp4_static_mse_sweep(w, amax0, global_amax, mult, fp8_max_norm=448.0, loss_out=None):

@@ -25,6 +25,7 @@ GPTQ_T = "tests/test_gpu_gptq.py"
 CALIB_T = "tests/test_gpu_calibrators.py"
 SEARCH_T = "tests/test_gpu_search_and_host.py"
 E2M1_T = "tests/test_gpu_e2m1_round.py"
+HESSIAN_T = "tests/test_gpu_hessian_sweep.py"
 
 _A32 = "x (and y) 32-byte aligned, vec_bytes unset"
 _A16 = "a pointer 16- but not 32-byte aligned, or vec_bytes=16"
@@ -348,7 +349,7 @@ LEDGER = {
     },
     "fp8_sweep_hessian_kernel": {
         "file": "search.cu", "entry": ("b200q_nvfp4_fp8_scale_sweep_hessian",),
-        "variants": (("b200q::fp8_sweep_hessian_kernel<{T}>", "always", "tests/test_gpu_modelopt_dropin.py"),),
+        "variants": (("b200q::fp8_sweep_hessian_kernel<{T}>", "always", HESSIAN_T),),
     },
     "nvfp4_static_mse_sweep_kernel": {
         "file": "search.cu", "entry": ("b200q_nvfp4_static_mse_sweep",),

@@ -23,24 +23,26 @@ FMT_FP8_EAGER = 4       # the reference's CPU FP8 rule (fl(1 / amax) * 448); ora
 PER_TENSOR_COL_BLOCK = 1 << 62
 
 
-def build() -> str:
-    """Compile (once per source digest) and return the library path."""
-    with open(_SRC, "rb") as f:
+def build(src: str = _SRC) -> str:
+    """Compile ``src`` (a C oracle under tools/, by default this one) once per source digest and return the library
+    path."""
+    name = os.path.splitext(os.path.basename(src))[0]
+    with open(src, "rb") as f:
         digest = hashlib.sha256(f.read() + " ".join(CFLAGS).encode()).hexdigest()[:16]
     for d in (os.path.join(os.path.dirname(_HERE), "build", "oracle"),
               os.path.join(tempfile.gettempdir(), f"b200q-oracle-{os.getuid()}")):
-        path = os.path.join(d, f"libgptq_oracle.{digest}.so")
+        path = os.path.join(d, f"lib{name}.{digest}.so")
         if os.path.exists(path):
             return path
         try:
             os.makedirs(d, exist_ok=True)
             tmp = f"{path}.{os.getpid()}.tmp"
-            subprocess.run(["cc", *CFLAGS, "-o", tmp, _SRC, "-lm"], check=True, capture_output=True)
+            subprocess.run(["cc", *CFLAGS, "-o", tmp, src, "-lm"], check=True, capture_output=True)
             os.replace(tmp, path)
             return path
         except (OSError, subprocess.CalledProcessError):
             continue
-    raise RuntimeError("could not compile tools/gptq_oracle.c")
+    raise RuntimeError(f"could not compile tools/{name}.c")
 
 
 def load():
