@@ -413,13 +413,22 @@ def _awq_block_size(weight, wq):
 
 
 def get_weight_scale(weight, block_size=None):
-    """model_calib.py:1453-1469: mean over rows of |W| / (blockamax + tiny), in the weight dtype."""
+    """model_calib.py:1453-1469: mean over rows of |W| / (blockamax + tiny), in the weight dtype.  A ragged last
+    block is zero-padded before its amax is taken, as in the reference."""
     if block_size and weight.shape[-1] % block_size == 0:
         sums = torch.zeros(weight.shape[-1], dtype=torch.float32, device=weight.device)
         ops.awq_weight_scale_sums_(sums, weight.contiguous(), block_size)
         return (sums / weight.shape[0]).to(weight.dtype).to(torch.float32)
+    cin = weight.shape[-1]
     w = weight.abs()
-    return (w / (w.amax(dim=1, keepdim=True) + torch.finfo(weight.dtype).tiny)).mean(0).to(torch.float32)
+    if block_size:
+        w = F.pad(w, (0, (-cin) % block_size))
+        shape = w.shape
+        w = w.reshape(-1, block_size)
+        scale = (w / (w.amax(dim=1, keepdim=True) + torch.finfo(weight.dtype).tiny)).reshape(shape)[..., :cin]
+    else:
+        scale = w / (w.amax(dim=1, keepdim=True) + torch.finfo(weight.dtype).tiny)
+    return scale.mean(0).to(torch.float32)
 
 
 def get_act_scale_(acc, x):
@@ -509,31 +518,46 @@ def awq_lite(model: nn.Module, forward_loop: Callable, alpha_step: float = 0.1, 
             m.input_quantizer.load_calib_amax()
     state["cache"] = False
     forward_loop(model)  # pass 2: search
+    def collapse_input_amax(m):
+        """Per-channel input amax of the cache pass -> per-tensor, the per-channel one kept for smoothing."""
+        iq = m.input_quantizer
+        if iq.amax is not None:
+            act_amax = iq.amax
+            iq._amax_for_smoothing = act_amax.cpu()
+            iq.reset_amax()
+            iq.axis = None
+            iq.amax = act_amax.amax()
+        iq.enable()
+
     for name, m in mods:
         st = m.awq_lite
         m.forward = m._b200_orig_forward
         del m._b200_orig_forward
-        for q in (m.weight_quantizer, m.input_quantizer):
-            if hasattr(q, "_pre_quant_scale"):
-                delattr(q, "_pre_quant_scale")
-        if st.is_input_quantized:
-            iq = m.input_quantizer
-            if iq.amax is not None:
-                act_amax = iq.amax
-                iq._amax_for_smoothing = act_amax.cpu()
-                iq.reset_amax()
-                iq.axis = None
-                iq.amax = act_amax.amax()
-            iq.enable()
-        ok = st.num_cache_steps > 0 and st.num_search_steps > 0 and not bool(torch.isnan(st.act_scale).any())
+        if st.num_cache_steps > 0 and st.num_search_steps == 0:
+            warnings.warn(f"awq_lite: Calling `forward_loop(model)` the second time did not forward data through the"
+                          f" {name}. Please provide a valid `forward_loop` function that can be used to forward data"
+                          " through the model many times.")
+        ok = (st.num_cache_steps > 0 and st.num_search_steps > 0 and not bool(torch.isnan(st.act_scale).any())
+              and not bool(torch.isnan(st.weight_scale).any()))
         if ok:
+            for q in (m.weight_quantizer, m.input_quantizer):
+                if hasattr(q, "_pre_quant_scale"):
+                    delattr(q, "_pre_quant_scale")
+            if st.is_input_quantized:
+                collapse_input_amax(m)
             losses = st.loss.tolist()
             st.best_alpha = st.alphas[min(range(len(losses)), key=losses.__getitem__)]
             st.best_scale = get_scale(st.act_scale, st.weight_scale, st.best_alpha)
             apply_pre_quant_scale_and_smooth(m, 1.0 / st.best_scale)
         else:
+            # model_calib.py:1673-1714: max calibration (the input quantizer is still disabled) and a neutral all-ones
+            # pre_quant_scale, so that export sees the same AWQ format on every linear
             warnings.warn(f"awq_lite: Disabling for {name}, quantizing with max calibration.")
             max_calibrate(m, lambda mod: mod.weight_quantizer(mod.weight))
+            m.input_quantizer.pre_quant_scale = torch.ones(m.weight.shape[1], dtype=m.weight.dtype,
+                                                           device=m.weight.device)
+            if st.is_input_quantized:
+                collapse_input_amax(m)
         if not debug:
             delattr(m, "awq_lite")
     _finalize_static_nvfp4(model)
@@ -547,37 +571,59 @@ def awq_clip(model: nn.Module, forward_loop: Callable, max_co_batch_size: int = 
 
     For every shrink ratio the weight is fake-quantized with ``amax * shrink`` (the fused kernels) and the
     per-block partial outputs ``sum_block(x * w)`` of up to ``max_tokens_per_batch`` tokens are compared
-    with the unquantized ones; the ratio with the smallest accumulated squared error wins per block."""
-    import math
+    with the unquantized ones; the ratio with the smallest accumulated squared error wins per block.
 
+    Like the reference:
+      * only weights with ``block_sizes`` are searched (a dynamic-block weight, e.g. NVFP4, clips its per-tensor
+        amax); every other quantizer -- per-channel INT8 or per-tensor FP8 weights too -- is max-calibrated by the
+        same forward loop;
+      * an input quantizer that was enabled is max-calibrated on every batch and stays disabled during the loop,
+        so the search sees unquantized inputs;
+      * a searched weight quantizer is disabled during the loop and re-enabled with its best amax only when its
+        linear saw tokens.  A linear the loop never reaches keeps its max amax and stays disabled (with its input
+        quantizer), as the reference leaves it.
+    The weight amax keeps the weight dtype (no fp32 promotion: the reference's awq_clip does not promote)."""
     assert forward_loop is not None, "forward_loop must be provided for awq_clip"
-    mods = [(n, m) for n, m in model.named_modules() if is_quantized_linear(m) and m.weight_quantizer.is_enabled]
+    mods = [(n, m) for n, m in model.named_modules() if is_quantized_linear(m) and m.weight_quantizer.is_enabled
+            and m.weight_quantizer.block_sizes is not None]
     ratios = [round(float(k), 2) for k in torch.arange(min_clip_ratio, 1.0, shrink_step)] + [1.0]
     for _, m in mods:
         wq = m.weight_quantizer
         wq.reset_amax()
-        max_calibrate(wq, lambda q, w=m.weight: q(w), distributed_sync=False)
+        enable_stats_collection(wq)
+        wq(m.weight)
+        finish_stats_collection(wq)
         st = type("AWQClipState", (), {})()
         st.w_amax = wq.amax.clone()
         st.block_size = _awq_block_size(m.weight, wq)
-        st.per_tensor = wq.axis is None and (wq.block_sizes is None or wq.block_sizes.get("type") == "dynamic")
+        st.per_tensor = wq.axis is None and wq.block_sizes.get("type") == "dynamic"
+        st.num_tokens = 0
+        st.is_input_quantized = m.input_quantizer.is_enabled
         co, ci = m.weight.shape
         shape = () if st.per_tensor else (co, math.ceil(ci / st.block_size))
         st.loss = {k: torch.zeros(shape, device=m.weight.device) for k in ratios}
         m.awq_clip = st
+        wq.disable()
 
         def fwd(self, x, _ratios=ratios):
-            st, wq = self.awq_clip, self.weight_quantizer
-            inputs = self.input_quantizer(x)
+            st, wq, iq = self.awq_clip, self.weight_quantizer, self.input_quantizer
+            if st.is_input_quantized:                # model_calib.py:1873-1876
+                iq.enable()
+                max_calibrate(iq, lambda q: q(x), distributed_sync=False)
+                iq.disable()
+            inputs = x
             w = self.weight
+            wq.enable()
             if st.per_tensor:
                 out_actual = inputs @ w.T
+                st.num_tokens += inputs.shape[0]
                 for shrink in _ratios:
                     wq.amax = st.w_amax * shrink
                     st.loss[shrink] += ((inputs @ wq(w).T) - out_actual).float().pow(2).mean()
             else:
                 xs = inputs.reshape(-1, inputs.shape[-1])
                 xs = xs[0:: max(1, xs.shape[0] // max_tokens_per_batch)]
+                st.num_tokens += xs.shape[0]
                 bs, (co, ci) = st.block_size, w.shape
                 pad = (-ci) % bs
                 wp = F.pad(w, (0, pad)) if pad else w
@@ -593,26 +639,39 @@ def awq_clip(model: nn.Module, forward_loop: Callable, max_co_batch_size: int = 
                         cur = (F.pad(cur, (0, pad)) if pad else cur).reshape(wb.shape)
                         st.loss[shrink][c0:c1] += ((xb * cur).sum(dim=-1) - org).float().pow(2).mean(dim=1)
             wq.amax = st.w_amax
+            wq.disable()
             return F.linear(x, w, self.bias)
 
         m._b200_orig_forward = m.forward
         m.forward = fwd.__get__(m, type(m))
-    forward_loop(model)
+    # the loop also max-calibrates every other quantizer (model_calib.py:1911-1920)
+    enable_stats_collection(model)
+    try:
+        forward_loop(model)
+    finally:
+        for _, m in mods:
+            m.forward = m._b200_orig_forward
+            del m._b200_orig_forward
+    if b200_dist.is_initialized():
+        b200_dist.sync_calibrator_amax(model)
+    finish_stats_collection(model)
     for _, m in mods:
         st = m.awq_clip
-        m.forward = m._b200_orig_forward
-        del m._b200_orig_forward
-        best_loss = torch.full_like(st.w_amax.float(), float("inf"))
-        best = torch.zeros_like(st.w_amax)
-        for shrink, loss in st.loss.items():
-            loss = loss.reshape(st.w_amax.shape)
-            better = loss < best_loss
-            best_loss = torch.where(better, loss, best_loss)
-            best = torch.where(better, st.w_amax * shrink, best)
-        m.weight_quantizer.amax = best
+        if st.num_tokens > 0:                        # postprocess (model_calib.py:1922-1935)
+            best_loss = torch.full_like(st.w_amax.float(), float("inf"))
+            best = torch.zeros_like(st.w_amax)
+            for shrink, loss in st.loss.items():
+                loss = loss.reshape(st.w_amax.shape)
+                better = loss < best_loss
+                best_loss = torch.where(better, loss, best_loss)
+                best = torch.where(better, st.w_amax * shrink, best)
+            st.best_clip_val = best
+            m.weight_quantizer.amax = best
+            m.weight_quantizer.enable()
+            if st.is_input_quantized:
+                m.input_quantizer.enable()
         if not debug:
             delattr(m, "awq_clip")
-    _finalize_static_nvfp4(model)
 
 
 # ---- GPTQ ------------------------------------------------------------------------------------------
