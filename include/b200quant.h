@@ -170,6 +170,16 @@ int b200q_nvfp4_block_log2_hist(const void *x, int dtype, size_t n_blocks, float
                                 float log2_max, int nbins, long long *hist,
                                 float *running_max_slot, b200q_stream_t stream);
 
+/* b200q_nvfp4_block_log2_hist over a table of tensors in ONE launch (descs: the MultiDesc table of
+ * b200q_amax_per_tensor_multi with n_units = 16-element blocks and first_cta counted in tiles of 512 blocks):
+ * entry i adds its counts to row slot_i of hist ([n_slots][nbins], int64) and its block amax maximum to
+ * running_max[slot_i] (fp32 bits, unsigned atomic max: NaN wins as in the per-tensor call).  Entries that share a
+ * slot accumulate into it.  Counts and running maxima equal those of one b200q_nvfp4_block_log2_hist call per entry.
+ * No host synchronisation and no allocation (graph-capturable). */
+int b200q_nvfp4_block_log2_hist_multi(const void *descs, int n_desc, size_t total_ctas, int dtype, float log2_min,
+                                      float log2_max, int nbins, long long *hist, float *running_max,
+                                      b200q_stream_t stream);
+
 /* Convert fp32 amax slots to `dtype` (the reference keeps _amax in the input dtype,
  * calib/max.py:64) and/or reset slots.  dst may be NULL (reset only). */
 int b200q_amax_export(const float *amax_slots, size_t n, void *dst, int dtype,

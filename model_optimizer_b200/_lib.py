@@ -48,6 +48,7 @@ _SIGNATURES = {
     "b200q_histogram_ex": [_P, c_int, c_size_t, c_int, _P, c_int, _P, _P, _P, _P],
     "b200q_amax_export": [_P, c_size_t, _P, c_int, _P],
     "b200q_nvfp4_block_log2_hist": [_P, c_int, c_size_t, c_float, c_float, c_int, _P, _P, _P],
+    "b200q_nvfp4_block_log2_hist_multi": [_P, c_int, c_size_t, c_int, c_float, c_float, c_int, _P, _P, _P],
     "b200q_fake_quant_int": [_P, _P, c_int, c_size_t, _P, c_int, c_size_t, c_size_t, c_int, c_int, c_int, _P],
     "b200q_fake_quant_fp8": [_P, _P, c_int, c_size_t, _P, c_int, c_size_t, c_size_t, _P],
     "b200q_fake_quant_fp8_eager": [_P, _P, c_int, c_size_t, _P, c_int, c_size_t, c_size_t, _P],

@@ -22,7 +22,11 @@ SURVEY.md 8(b), plus the module-level functions the hooks cannot reach.
      pre-computed block scales, ``keep_high_precision``) are handed back to the host application's own function;
    * ``normalized_hadamard_transform`` as named in ``nn/modules/tensor_quantizer.py`` (:67, called by
      ``_rotate_inputs`` :664-668): every ``rotate`` config on CUDA tensors runs ``b200q_hadamard`` instead of needing
-     the external ``fast_hadamard_transform`` package (other inputs go to the host application's own function).
+     the external ``fast_hadamard_transform`` package (other inputs go to the host application's own function);
+   * ``NVFP4ActHeadroomCalibrator`` as named in ``model_calib.py`` (constructed directly by ``nvfp4_act_headroom``):
+     a subclass whose ``collect`` is one ``b200q_nvfp4_block_log2_hist`` launch for CUDA inputs in fp32 / fp16 /
+     bf16 with blocks of 16 (the reference: a clone, two reductions, a host-synchronising compaction, ``log2`` and
+     ``bincount`` per batch); other inputs run the reference's own methods.
 6. ``register_gptq_helper("b200", B200GPTQHelper)`` (utils/calib_utils.py:316-326): ``gptq`` builds this
    ``GPTQHelper`` subclass for weight quantizers on the b200 backend.  Its ``_blockwise_update`` runs the GPTQ column
    kernel (``b200q_gptq_block``, one launch per block, plus the reference's trailing ``addmm_``) for the formats the
@@ -277,6 +281,54 @@ def _make_mse_factory(base, ref_mse_cls):
     return B200MseCalibrator
 
 
+def _make_headroom_calibrator(ref_cls):
+    from .calib.nvfp4_act_headroom import NVFP4ActHeadroomCalibrator as Mine
+
+    class B200NVFP4ActHeadroomCalibrator(ref_cls):
+        """Stands in for ``NVFP4ActHeadroomCalibrator`` in ``nvfp4_act_headroom_calibrate`` (a subclass, so
+        ``isinstance`` checks keep holding; the reference's constructor validates the arguments).  CUDA inputs in fp32 /
+        fp16 / bf16 with blocks of 16 go to this engine's calibrator; a NaN or inf block then raises in
+        ``compute_amax`` rather than in the ``collect`` of its batch, which would cost a host sync per batch.  Batches
+        that ran the reference's ``collect`` (other inputs) are merged with the engine's statistic before the amax."""
+
+        def __init__(self, num_bits=(2, 1), axis=None, unsigned=False, *, block_size=16, anchor_percentile=1.0,
+                     upper_percentile=99.99, rho=16384.0, num_bins=512, log2_min=-40.0, log2_max=40.0):
+            kw = dict(anchor_percentile=anchor_percentile, upper_percentile=upper_percentile, rho=rho,
+                      num_bins=num_bins, log2_min=log2_min, log2_max=log2_max)
+            super().__init__(num_bits, axis, unsigned, block_size=block_size, **kw)
+            self._b200 = Mine(num_bits, axis, unsigned, block_size=16, **kw) if block_size == 16 else None
+
+        def collect(self, x):
+            if self._b200 is None or not x.is_cuda or x.dtype not in ops._DT:
+                return super().collect(x)
+            stats["calib.nvfp4_act_headroom"] += 1
+            return self._b200.collect(x)
+
+        def compute_amax(self):
+            if self._b200 is None or self._b200._hist is None:
+                return super().compute_amax()
+            stats["calib.nvfp4_act_headroom"] += 1
+            if self._running_max is None:
+                return self._b200.compute_amax()
+            rmax = self._b200._running_max.reshape(()).to(self._running_max.device)
+            if not bool(torch.isfinite(rmax)):
+                raise AssertionError("detected nan/inf values in amax")
+            self._running_max = torch.maximum(self._running_max, rmax)
+            if int(self._b200._hist.sum()) > 0:
+                h = self._b200._hist.to(self._running_max.device)
+                self._hist = h if self._hist is None else self._hist + h
+            self._b200.reset()
+            return super().compute_amax()
+
+        def reset(self):
+            if self._b200 is not None:
+                stats["calib.nvfp4_act_headroom"] += 1
+                self._b200.reset()
+            super().reset()
+
+    return B200NVFP4ActHeadroomCalibrator
+
+
 def _make_gptq_helper(ref_helper_cls):
     class B200GPTQHelper(ref_helper_cls):
         """``GPTQHelper`` whose blockwise update runs ``ops.gptq_blockwise_update`` for quantizers inside the GPTQ
@@ -372,10 +424,12 @@ def install(patch_extensions: bool = True, patch_functions: bool = True):
                         "nvfp4_quantize": NVFP4QTensor.__dict__["quantize"],
                         "fp8_quantize": FP8QTensor.__dict__["quantize"],
                         "mse": ref_model_calib.MseCalibrator,
+                        "headroom": ref_model_calib.NVFP4ActHeadroomCalibrator,
                         "hadamard": orig_hadamard}
         ref_tq.static_blockwise_fp4_fake_quant = static_fp4
         ref_tq.normalized_hadamard_transform = hadamard
         ref_model_calib.MseCalibrator = _make_mse_factory(base, ref_model_calib.MseCalibrator)
+        ref_model_calib.NVFP4ActHeadroomCalibrator = _make_headroom_calibrator(ref_model_calib.NVFP4ActHeadroomCalibrator)
         NVFP4QTensor.quantize, FP8QTensor.quantize = _make_qtensor_patches(NVFP4QTensor, FP8QTensor)
     return B200MaxCalibrator, B200HistogramCalibrator
 
@@ -395,6 +449,7 @@ def uninstall():
         ref_tq.static_blockwise_fp4_fake_quant = fn["static"]
         ref_tq.normalized_hadamard_transform = fn["hadamard"]
         ref_model_calib.MseCalibrator = fn["mse"]
+        ref_model_calib.NVFP4ActHeadroomCalibrator = fn["headroom"]
         NVFP4QTensor.quantize = fn["nvfp4_quantize"]
         FP8QTensor.quantize = fn["fp8_quantize"]
 

@@ -14,9 +14,8 @@ import torch
 import torch.nn.functional as F
 
 from .. import ops
+from ..config import FP8_NORMAL_DYNAMIC_RANGE as _FP8_NORMAL_DYNAMIC_RANGE
 from .calibrator import _Calibrator
-
-_FP8_NORMAL_DYNAMIC_RANGE = 448.0 / 2.0**-6
 _ANCHOR_FLOOR_RATIO = 1e6
 
 
@@ -73,23 +72,28 @@ class NVFP4ActHeadroomCalibrator(_Calibrator):
         idx = int(torch.searchsorted(cdf, percentile / 100.0 * total).clamp(0, self._num_bins - 1).item())
         return float(2.0 ** (self._log2_min + (idx + 0.5) / self._num_bins * (self._log2_max - self._log2_min)))
 
-    @torch.no_grad()
-    def compute_amax(self):
-        if self._hist is None:
-            return None
-        rmax = self._running_max.reshape(())
-        if not bool(torch.isfinite(rmax)):
+    def amax_from_host(self, counts: torch.Tensor, rmax: float):
+        """``compute_amax`` on host values -- ``counts`` a CPU copy of the histogram, ``rmax`` the running max -- as a
+        Python float (exact in fp32), or None.  Lets a caller that holds many histograms copy them in one transfer."""
+        if not math.isfinite(rmax):
             raise AssertionError("detected nan/inf values in amax")
-        if int(self._hist.sum()) == 0:
-            return None if float(rmax) == 0 else rmax.clone()
-        counts = self._hist.float().cpu()
-        upper = float(rmax) if self._upper_percentile >= 100.0 else self._percentile(counts, self._upper_percentile)
+        if int(counts.sum()) == 0:
+            return None if rmax == 0 else rmax
+        counts = counts.float()
+        upper = rmax if self._upper_percentile >= 100.0 else self._percentile(counts, self._upper_percentile)
         anchor = self._percentile(counts, self._anchor_percentile, upper / _ANCHOR_FLOOR_RATIO if upper else None) \
             if upper else None
         if not upper or upper <= 0 or not anchor or anchor <= 0:
-            return rmax.clone()
+            return rmax
         headroom = self._rho * anchor
         if headroom <= upper:
             warnings.warn(f"[nvfp4_act_headroom] per-block amax range {upper / anchor:.1f} leaves no headroom at "
                           f"rho={self._rho:g}; the scale falls back to the top of the calibrated range.")
-        return torch.tensor(max(headroom, upper), dtype=torch.float32, device=self._hist.device)
+        return max(headroom, upper)
+
+    @torch.no_grad()
+    def compute_amax(self):
+        if self._hist is None:
+            return None
+        amax = self.amax_from_host(self._hist.cpu(), float(self._running_max.reshape(())))
+        return None if amax is None else torch.tensor(amax, dtype=torch.float32, device=self._hist.device)

@@ -134,6 +134,43 @@ class GPTQCalibConfig:
         return bool(lw.get("enable", False)) if isinstance(lw, dict) else bool(lw)
 
 
+# NVFP4ActHeadroomCalibrator: rho must stay below the FP8-E4M3 normal dynamic range, 448 / 2^-6
+FP8_NORMAL_DYNAMIC_RANGE = 448.0 / 2.0**-6
+_WEIGHT_SCALE_METHODS = ("max", "mse", "local_hessian")
+
+
+@dataclass
+class NVFP4ActHeadroomCalibConfig:
+    """quantization/config.py:1257-1330: the per-tensor global scale of every NVFP4 input quantizer from the
+    distribution of its per-block amaxes, ``max(rho * P_anchor, P_upper)``, which leaves headroom above the calibrated
+    range.  ``weight_scale_algorithm`` calibrates the weights (and runs the max pass that collects the histograms):
+    ``None`` means ``{"method": "max"}``; otherwise a dict whose ``method`` is ``max``, ``mse`` or ``local_hessian``, plus
+    that algorithm's own options."""
+
+    method: str = "nvfp4_act_headroom"
+    anchor_percentile: float = 1.0
+    upper_percentile: float = 99.99
+    rho: float = 16384.0
+    weight_scale_algorithm: dict | None = None
+
+    def __post_init__(self):
+        if self.method != "nvfp4_act_headroom":
+            raise ValueError(f"method must be 'nvfp4_act_headroom', got {self.method!r}")
+        for name in ("anchor_percentile", "upper_percentile"):
+            v = getattr(self, name)
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not (0.0 < v <= 100.0):
+                raise ValueError(f"{name} must be in (0, 100], got {v!r}")
+        r = self.rho
+        if isinstance(r, bool) or not isinstance(r, (int, float)) or not (0.0 < r < FP8_NORMAL_DYNAMIC_RANGE):
+            raise ValueError(f"rho must be in (0, {FP8_NORMAL_DYNAMIC_RANGE:g}), got {r!r}")
+        w = self.weight_scale_algorithm
+        if w is None:
+            self.weight_scale_algorithm = {"method": "max"}
+        elif not isinstance(w, dict) or w.get("method") not in _WEIGHT_SCALE_METHODS:
+            raise ValueError(f"weight_scale_algorithm must be None or a dict whose method is one of "
+                             f"{_WEIGHT_SCALE_METHODS}, got {w!r}")
+
+
 _DEFAULT_DISABLED = [
     "*block_sparse_moe.gate*", "*linear_attn.conv1d*", "*linear_attn.in_proj_a*", "*linear_attn.in_proj_b*",
     "*lm_head*", "*mixer.conv1d*", "*mlp.gate.*", "*mlp.shared_expert_gate.*", "*output_layer*", "*proj_out.*",

@@ -517,27 +517,75 @@ static int launch_histogram(const void *x, size_t n, int take_abs, const float *
 // ---------------------------------------------------------------------------------------------
 // NVFP4 activation headroom: log2 histogram of per-block amax (calib/nvfp4_act_headroom.py:110-149)
 // ---------------------------------------------------------------------------------------------
+// One tensor (descs == nullptr): a grid-stride loop over its n_blocks blocks into hist / max_slot.  A table of tensors
+// (descs: MultiDesc, unit = 16-element block, first_cta counted in tiles of kHistThreads = 512 blocks, as
+// ops.TensorTable builds it; n_blocks = the table's tile count): CTA c takes tiles 2c and 2c + 1, each found by binary
+// search and counted in a shared-memory histogram of its own, so every thread has two block loads in flight; tile t's
+// counts / running max go to row slot_t of hist ([n_slots][nbins]) and max_slot[slot_t], and entries sharing a slot
+// accumulate.  Both launches bin through the same code, so the grouped launch bins every block exactly as the
+// per-tensor one does.
+constexpr int kHistTilesPerCta = 2;
+
 template <typename Tag, int VB>
 __global__ void __launch_bounds__(kHistThreads)
-    block_log2_hist_kernel(const uint8_t *__restrict__ x, size_t n_blocks, float log2_min, float range,
-                           int nbins, unsigned long long *__restrict__ hist, uint32_t *__restrict__ max_slot) {
-  extern __shared__ uint32_t s_hist[];
-  for (int b = threadIdx.x; b < nbins; b += kHistThreads) s_hist[b] = 0u;
-  __syncthreads();
+    block_log2_hist_kernel(const uint8_t *__restrict__ x, size_t n_blocks, const MultiDesc *__restrict__ descs,
+                           int n_desc, float log2_min, float range, int nbins, unsigned long long *__restrict__ hist,
+                           uint32_t *__restrict__ max_slot) {
+  extern __shared__ uint32_t s_hist[];                    // [1 or kHistTilesPerCta][nbins]
+  const int n_hist = descs != nullptr ? kHistTilesPerCta : 1;
+  for (int b = threadIdx.x; b < n_hist * nbins; b += kHistThreads) s_hist[b] = 0u;
   const float fbins = (float)nbins;
-  uint32_t mx = 0;
-  for (size_t i = (size_t)blockIdx.x * kHistThreads + threadIdx.x; i < n_blocks; i += (size_t)gridDim.x * kHistThreads) {
-    Block<Tag, VB> b;
-    b.load(x, i);
+  // bins block b into the histogram h; returns its amax as fp32 bits
+  auto bin_block = [&](Block<Tag, VB> &b, uint32_t *h) -> uint32_t {
     const uint32_t fb = Elem<Tag>::absbits_to_f32bits(b.absmax_native_bits());
-    mx = max(mx, fb);
     const float v = __uint_as_float(fb);
     if (v > 0.0f) {  // NaN fails the test and only shows up in the running max
       const float frac = __fdiv_rn(__fsub_rn(log2f(v), log2_min), range);
       long long idx = (long long)floorf(__fmul_rn(frac, fbins));
       idx = idx < 0 ? 0 : (idx > nbins - 1 ? nbins - 1 : idx);
-      atomicAdd(&s_hist[(int)idx], 1u);
+      atomicAdd(&h[(int)idx], 1u);
     }
+    return fb;
+  };
+  if (descs != nullptr) {
+    const size_t t0 = (size_t)blockIdx.x * kHistTilesPerCta;
+    Block<Tag, VB> blk[kHistTilesPerCta];
+    long long slot[kHistTilesPerCta];
+    bool have[kHistTilesPerCta];                           // this thread holds a block of tile t0 + u
+#pragma unroll
+    for (int u = 0; u < kHistTilesPerCta; ++u) {
+      have[u] = false;
+      if (t0 + u >= n_blocks) continue;                   // uniform over the CTA: the table's last CTA may hold one tile
+      const MultiDesc d = descs[multi_find(descs, n_desc, t0 + u)];
+      const size_t i = (t0 + u - d.first_cta) * kHistThreads + threadIdx.x;
+      slot[u] = d.slot;
+      have[u] = i < d.n_units;
+      if (have[u]) blk[u].load(d.x, i);                    // both loads issued before either block is binned
+    }
+    __syncthreads();
+    uint32_t mx[kHistTilesPerCta];
+#pragma unroll
+    for (int u = 0; u < kHistTilesPerCta; ++u) mx[u] = have[u] ? bin_block(blk[u], s_hist + u * nbins) : 0u;
+#pragma unroll
+    for (int u = 0; u < kHistTilesPerCta; ++u) {
+      if (t0 + u >= n_blocks) break;
+      const uint32_t m = block_max<kHistThreads>(mx[u]);
+      if (threadIdx.x == 0 && m != 0u) atomicMax(max_slot + slot[u], m);
+      __syncthreads();                                     // block_max's scratch is reused by the next tile; bins complete
+      unsigned long long *row = hist + (size_t)slot[u] * (size_t)nbins;
+      for (int b = threadIdx.x; b < nbins; b += kHistThreads) {
+        const uint32_t c = s_hist[u * nbins + b];
+        if (c) atomicAdd(&row[b], (unsigned long long)c);
+      }
+    }
+    return;
+  }
+  __syncthreads();
+  uint32_t mx = 0;
+  for (size_t i = (size_t)blockIdx.x * kHistThreads + threadIdx.x; i < n_blocks; i += (size_t)gridDim.x * kHistThreads) {
+    Block<Tag, VB> b;
+    b.load(x, i);
+    mx = max(mx, bin_block(b, s_hist));
   }
   mx = block_max<kHistThreads>(mx);
   if (threadIdx.x == 0 && mx != 0u) atomicMax(max_slot, mx);
@@ -573,11 +621,33 @@ extern "C" int b200q_nvfp4_block_log2_hist(const void *x, int dtype, size_t n_bl
   do {                                                                                             \
     auto kern = block_log2_hist_kernel<Tag, VB_>;                                                  \
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-    kern<<<(unsigned)grid, kHistThreads, smem, st>>>(xb, n_blocks, log2_min, range, nbins, h, ms);  \
+    kern<<<(unsigned)grid, kHistThreads, smem, st>>>(xb, n_blocks, nullptr, 0, log2_min, range, nbins, h, ms); \
   } while (0)
   B200Q_DISPATCH_DTYPE(dtype, Tag, if (ax % 32 == 0) LAUNCH(32); else LAUNCH(16));
 #undef LAUNCH
   return check_launch("block_log2_hist_kernel");
+}
+
+extern "C" int b200q_nvfp4_block_log2_hist_multi(const void *descs, int n_desc, size_t total_ctas, int dtype,
+                                                 float log2_min, float log2_max, int nbins, long long *hist,
+                                                 float *running_max, b200q_stream_t stream) {
+  if (n_desc == 0 || total_ctas == 0) return B200Q_OK;
+  B200Q_REQUIRE(descs != nullptr && hist != nullptr && running_max != nullptr && n_desc > 0, "null pointer");
+  B200Q_REQUIRE(nbins > 0 && nbins <= 16384 && log2_max > log2_min, "bad histogram arguments");
+  B200Q_REQUIRE(total_ctas <= 0x7fffffffu, "too many CTAs");
+  const size_t smem = (size_t)kHistTilesPerCta * nbins * sizeof(uint32_t);   // one histogram per tile of a CTA
+  const size_t grid = (total_ctas + kHistTilesPerCta - 1) / kHistTilesPerCta;
+  const float range = log2_max - log2_min;
+  const MultiDesc *dd = static_cast<const MultiDesc *>(descs);
+  unsigned long long *h = reinterpret_cast<unsigned long long *>(hist);
+  uint32_t *ms = reinterpret_cast<uint32_t *>(running_max);
+  cudaStream_t st = (cudaStream_t)stream;
+  B200Q_DISPATCH_DTYPE(dtype, Tag, {
+    auto kern = block_log2_hist_kernel<Tag, 32>;          // table entries are 32-byte aligned (ops.TensorTable)
+    if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    kern<<<(unsigned)grid, kHistThreads, smem, st>>>(nullptr, total_ctas, dd, n_desc, log2_min, range, nbins, h, ms);
+  });
+  return check_launch("block_log2_hist_kernel<grouped>");
 }
 
 extern "C" int b200q_histogram(const void *x, int dtype, size_t n, int take_abs,

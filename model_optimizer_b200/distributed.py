@@ -155,4 +155,32 @@ def sync_calibrator_amax(model, group=None, include_weights=True) -> int:
     return len(arena)
 
 
-__all__ = ["AmaxArena", "is_initialized", "shard_layers", "sync_calibrator_amax"]
+def sync_headroom_amax(model, group=None) -> int:
+    """MAX-merge, across the ranks of ``group``, the ``_amax`` of every enabled quantizer whose calibrator is an
+    ``NVFP4ActHeadroomCalibrator`` -- after the amaxes are loaded, since a headroom amax is a percentile rule, not a
+    running max that ``sync_calibrator_amax`` could merge slot by slot.  One all-reduce over a flat fp32 buffer
+    (``named_modules`` order, zeros where a rank holds no amax): the result is the largest per-rank scale
+    (quantization/model_calib.py:606-609).  A quantizer that holds no amax here adopts a positive merged one.  Returns
+    the number of quantizers merged."""
+    from .calib import NVFP4ActHeadroomCalibrator
+    from .nn import TensorQuantizer
+
+    qs = [q for _, q in model.named_modules()
+          if isinstance(q, TensorQuantizer) and not q._disabled and isinstance(q._calibrator, NVFP4ActHeadroomCalibrator)]
+    if not qs:
+        return 0
+    device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" \
+        else torch.device("cpu")
+    zero = torch.zeros((), dtype=torch.float32, device=device)
+    buf = torch.stack([q._amax.detach().reshape(()).to(device, torch.float32) if hasattr(q, "_amax") else zero
+                       for q in qs])
+    dist.all_reduce(buf, op=dist.ReduceOp.MAX, group=group)
+    for q, v in zip(qs, buf):
+        if hasattr(q, "_amax"):
+            q._amax.copy_(v.reshape(q._amax.shape))
+        elif float(v) > 0:
+            q.amax = v.clone()
+    return len(qs)
+
+
+__all__ = ["AmaxArena", "is_initialized", "shard_layers", "sync_calibrator_amax", "sync_headroom_amax"]

@@ -10,6 +10,10 @@ Drives the three numeric hot paths for a whole decoder-only model whose linears 
   fake quant: every input quantizer runs its fused fake-quant forward (NVFP4 / FP8 / INT8);
   weights   : per-tensor amax + quant-and-pack of every owned weight.
 
+``calib="nvfp4_act_headroom"`` (NVFP4, one GPU) calibrates with the NVFP4 activation-headroom rule instead of max:
+collect adds every activation's per-block log2 histogram and running max to one ``[n_quantizers, 512]`` int64 table
+(one grouped launch), and ``finish`` turns each histogram into an fp32 amax on the host, once per job.
+
 Decoder layers are sharded contiguously over ranks (``distributed.shard_layers``); the statistics of
 different layers are independent, so the only collective is the arena all-reduce -- ONE per calibration job
 (``allreduce_every`` batches, 64 for 512 samples x batch 8), issued on a communication stream.  The ranks form a
@@ -30,8 +34,8 @@ from dataclasses import dataclass
 import torch
 
 from . import ops
-from .calib import MaxCalibrator
-from .config import QuantizerAttributeConfig
+from .calib import MaxCalibrator, NVFP4ActHeadroomCalibrator
+from .config import NVFP4ActHeadroomCalibConfig, QuantizerAttributeConfig
 from .distributed import AmaxArena, shard_layers
 from .nn import TensorQuantizer
 
@@ -74,7 +78,21 @@ class ShardedPTQEngine:
 
     def __init__(self, plan: ModelPlan, tokens: int, qformat: str = "nvfp4", dtype=torch.bfloat16,
                  device="cuda", rank: int = 0, world_size: int = 1, group=None, allreduce_every: int = 64,
-                 handoff: bool = True, dedupe_shared_inputs: bool = False, grouped: bool = True):
+                 handoff: bool = True, dedupe_shared_inputs: bool = False, grouped: bool = True,
+                 calib: str = "max", headroom: dict | None = None):
+        """``calib``: ``"max"`` or ``"nvfp4_act_headroom"`` (NVFP4 and ``world_size == 1`` only); ``headroom``: the
+        ``anchor_percentile`` / ``upper_percentile`` / ``rho`` of the latter (``NVFP4ActHeadroomCalibConfig``)."""
+        if calib not in ("max", "nvfp4_act_headroom"):
+            raise ValueError(f"calib must be 'max' or 'nvfp4_act_headroom', got {calib!r}")
+        if calib == "nvfp4_act_headroom":
+            if qformat != "nvfp4":
+                raise ValueError("calib='nvfp4_act_headroom' calibrates NVFP4 input quantizers only")
+            if world_size > 1:
+                raise NotImplementedError("calib='nvfp4_act_headroom' runs on one GPU; a multi-GPU headroom engine "
+                                          "is not implemented")
+        elif headroom is not None:
+            raise ValueError("headroom options need calib='nvfp4_act_headroom'")
+        self.calib = calib
         self.plan, self.tokens, self.qformat, self.dtype = plan, tokens, qformat, dtype
         self.device = torch.device(device)
         self.rank, self.world_size, self.group = rank, world_size, group
@@ -99,6 +117,21 @@ class ShardedPTQEngine:
                 cal._shape, cal._dtype = (), dtype
                 q._amax = self.amax_arena[idx[qn]:idx[qn] + 1].view(())   # view: export fills it
                 self.quantizers.append((qn, q, cin))
+        self.hist = self.running_max = None
+        if calib == "nvfp4_act_headroom":
+            # every quantizer's histogram and running max are rows of one table (the grouped launch fills them all);
+            # its fp32 amax is its arena slot, which finish() writes and the fake quant reads as it is (no export)
+            hc = NVFP4ActHeadroomCalibConfig(**(headroom or {}))
+            n = len(self.quantizers)
+            self.hist = torch.zeros(n, 512, dtype=torch.int64, device=self.device)
+            self.running_max = torch.zeros(n, dtype=torch.float32, device=self.device)
+            for i, (qn, q, _) in enumerate(self.quantizers):
+                cal = NVFP4ActHeadroomCalibrator(anchor_percentile=hc.anchor_percentile,
+                                                 upper_percentile=hc.upper_percentile, rho=hc.rho)
+                cal._hist, cal._running_max, cal._dtype = self.hist[i], self.running_max[i:i + 1], dtype
+                q._calibrator = cal
+                q._amax = self.arena.view(qn).view(())
+        self._tables = {}
         self._graphs = {}
         self._graph_sets = []
         self.allreduce_every = max(1, int(allreduce_every))
@@ -204,9 +237,28 @@ class ShardedPTQEngine:
 
     # ---- the hot path ----------------------------------------------------------------------------------
     def collect(self, acts):
-        """Calibration collect of one batch: one fused |x|-max kernel per quantizer."""
+        """Calibration collect of one batch: one fused |x|-max kernel per quantizer.  Headroom mode: one grouped
+        histogram launch over every activation (``grouped``), else one calibrator collect per quantizer."""
+        if self.hist is not None and self.grouped:
+            ops.nvfp4_block_log2_hist_multi_(self.hist, self.running_max, self._cached_table(acts))
+            return
         for (_, q, _), x in zip(self.quantizers, acts):
             q._calibrator.collect(x)
+
+    def _cached_table(self, acts, ys=None):
+        """The descriptor table of these (static) buffers, built on first use -- outside any graph capture, since the
+        build copies the table to the device.  Slot i = quantizer i."""
+        key = (tuple(x.data_ptr() for x in acts), None if ys is None else tuple(y.data_ptr() for y in ys))
+        t = self._tables.get(key)
+        if t is None:
+            if ys is not None:
+                spans = sorted((y.data_ptr(), y.data_ptr() + y.numel() * y.element_size()) for y in ys)
+                if any(b[0] < a[1] for a, b in zip(spans, spans[1:])):
+                    raise ValueError("the grouped headroom fake quant needs non-overlapping outputs "
+                                     "(alloc_outputs(n_ring=len(engine.quantizers)))")
+            t = ops.TensorTable(acts, list(range(len(acts))), ys, "block16")
+            self._tables[key] = t
+        return t
 
     def _table(self, acts, outs, parity):
         """Descriptor table of a parity's static buffers for the fused collect + fake quant: every owned quantizer's
@@ -223,6 +275,14 @@ class ShardedPTQEngine:
 
     def _capture_set(self, acts, outs, parity, side):
         g_collect, g_export, g_fq = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
+        if self.hist is not None:
+            # headroom: the amax is not a running max, so the speculative fused pass cannot be fixed up; the step is
+            # collect, then fake quant with the amaxes of the last finish()
+            with torch.cuda.graph(g_collect, stream=side):
+                self.collect(acts)
+            with torch.cuda.graph(g_fq, stream=side):
+                self.fake_quant(acts, outs, parity)
+            return {"collect": g_collect, "fake_quant": g_fq}
         if self.grouped:
             # ONE read of every activation per step: the fused pass fake-quantizes with the amax exported by the
             # previous step while it collects; the fix-up redoes the (rare) entries whose exported amax changes.
@@ -258,7 +318,14 @@ class ShardedPTQEngine:
         return {"collect": g_collect, "export": g_export, "fake_quant": g_fq}
 
     def finish(self):
-        """One collective + one export kernel: arena (fp32) -> all quantizers' _amax (input dtype)."""
+        """One collective + one export kernel: arena (fp32) -> all quantizers' _amax (input dtype).  Headroom mode:
+        the histogram table comes to the host in one copy, every quantizer's amax is computed there, and the fp32
+        amaxes go to the arena slots the fake quant reads."""
+        if self.hist is not None:
+            counts, rmax = self.hist.cpu(), self.running_max.cpu().tolist()
+            amax = [q._calibrator.amax_from_host(counts[i], rmax[i]) for i, (_, q, _) in enumerate(self.quantizers)]
+            self.arena.freeze().copy_(torch.tensor([0.0 if a is None else a for a in amax], dtype=torch.float32))
+            return
         if self.world_size > 1:
             self.arena.all_reduce(self.group)
         self.export_amax()
@@ -272,6 +339,10 @@ class ShardedPTQEngine:
         the buffer this rank sends on (a stand-in for the layer output the GEMMs would produce)."""
         n = len(outs)
         res = []
+        if self.hist is not None and self.grouped:
+            ys = [outs[i % n][: x.numel()].view_as(x) for i, x in enumerate(acts)]
+            ops.fake_quant_nvfp4_multi(self._cached_table(acts, ys), self.arena.freeze())
+            return ys
         last_hidden = len(self.quantizers) - 4 if (self.handoff and self.hand_out is not None) else -1
         for i, ((_, q, _), x) in enumerate(zip(self.quantizers, acts)):
             out = self.hand_out[parity] if i == last_hidden else outs[i % n][: x.numel()].view_as(x)
@@ -289,6 +360,9 @@ class ShardedPTQEngine:
         self.amax_arena.zero_()
         if self.redo_count is not None:
             self.redo_count.zero_()
+        if self.hist is not None:
+            self.hist.zero_()
+            self.running_max.zero_()
 
     # ---- CUDA graphs -----------------------------------------------------------------------------------
     def capture(self, acts, outs):
@@ -298,8 +372,9 @@ class ShardedPTQEngine:
         side = torch.cuda.Stream(self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(side):
-            self.collect(acts)       # warm-up outside capture (module / kernel loading)
-            self.export_amax()
+            self.collect(acts)       # warm-up outside capture (module / kernel loading, descriptor tables)
+            if self.hist is None:
+                self.export_amax()
             self.fake_quant(acts, outs)
         torch.cuda.synchronize(self.device)
         self.reset()
@@ -373,7 +448,10 @@ class ShardedPTQEngine:
                 # the exchange issued one step ago (parity p) delivered this step's input and released hand_out[p]
                 main.wait_event(self._ev_comm[p])
             self._exchange(1 - p)                         # previous step's output travels under this step's kernels
-        if self.grouped:
+        if self.hist is not None:
+            g["collect"].replay()
+            g["fake_quant"].replay()
+        elif self.grouped:
             g["fake_quant"].replay()
             g["collect"].replay()
             g["export"].replay()
@@ -398,6 +476,8 @@ class ShardedPTQEngine:
             torch.cuda.current_stream(self.device).wait_stream(self._comm_stream)
 
     def launches_per_step(self) -> int:
+        if self.hist is not None:
+            return 2 if self.grouped else 2 * len(self.quantizers)
         return 3 if self.grouped else 2 * len(self.quantizers) + 1
 
     def act_bytes_per_step(self) -> tuple[int, int]:
@@ -406,7 +486,7 @@ class ShardedPTQEngine:
         (the live blocks of the pre-flagged output tiles it rewrites, ``ops.output_tiles``; known once captured)."""
         elems = sum(self.tokens * cin for _, _, cin in self.quantizers)
         es = torch.empty((), dtype=self.dtype).element_size()
-        return self._fixup_bytes if self.grouped else elems * es, 2 * elems * es
+        return self._fixup_bytes if self.grouped and self.hist is None else elems * es, 2 * elems * es
 
     # ---- weights -----------------------------------------------------------------------------------------
     def weight_pass(self, weights):

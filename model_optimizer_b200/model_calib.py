@@ -166,7 +166,55 @@ def max_calibrate(model: nn.Module, forward_loop: Callable | None = None, distri
     if distributed_sync and b200_dist.is_initialized():
         b200_dist.sync_calibrator_amax(model)
     finish_stats_collection(model)
+    if distributed_sync and b200_dist.is_initialized():
+        b200_dist.sync_headroom_amax(model)
     _finalize_static_nvfp4(model)
+
+
+def _is_nvfp4_dynamic_input_quantizer(name: str, q) -> bool:
+    """model_calib.py:501-529: an enabled, non-``_dynamic`` NVFP4 dynamic-block (E2M1, E4M3 scales) input quantizer."""
+    return (name.endswith("input_quantizer") and isinstance(q, TensorQuantizer) and not q._disabled
+            and not q._dynamic and q.is_nvfp4_dynamic)
+
+
+@torch.no_grad()
+def nvfp4_act_headroom_calibrate(model: nn.Module, forward_loop: Callable | None = None, *,
+                                 anchor_percentile: float = 1.0, upper_percentile: float = 99.99, rho: float = 16384.0,
+                                 weight_scale_algorithm: dict | None = None):
+    """model_calib.py:500-636: every NVFP4 dynamic-block input quantizer gets an ``NVFP4ActHeadroomCalibrator`` for
+    the run of ``weight_scale_algorithm`` (``max``, ``mse`` or ``local_hessian``; ``None`` is ``max``), whose max pass
+    collects the per-block log2 histograms and loads ``amax = max(rho * P_anchor, P_upper)`` (fp32) into those
+    quantizers; the original calibrators are restored afterwards.  Everything is validated before the model changes:
+    an NVFP4 input quantizer with blocks other than 16 raises ``NotImplementedError``.  Under data parallelism the
+    per-rank amaxes are merged with one MAX all-reduce (``distributed.sync_headroom_amax``): the largest per-rank
+    scale, as the reference documents."""
+    from .calib import NVFP4ActHeadroomCalibrator
+    from .config import NVFP4ActHeadroomCalibConfig
+
+    cfg = NVFP4ActHeadroomCalibConfig(anchor_percentile=anchor_percentile, upper_percentile=upper_percentile, rho=rho,
+                                      weight_scale_algorithm=weight_scale_algorithm)
+    targets = [(n, q) for n, q in _quantizers(model) if _is_nvfp4_dynamic_input_quantizer(n, q)]
+    for n, q in targets:
+        if q._block_sizes.get(-1, 16) != 16:
+            raise NotImplementedError(f"nvfp4_act_headroom: {n!r} quantizes blocks of {q._block_sizes.get(-1)}; "
+                                      f"only NVFP4 input blocks of 16 are supported")
+    weight_kw = {k: v for k, v in cfg.weight_scale_algorithm.items() if k != "method"}
+    weight_fn = {"max": max_calibrate, "mse": mse_calibrate,
+                 "local_hessian": local_hessian_calibrate}[cfg.weight_scale_algorithm["method"]]
+    if not targets:
+        warnings.warn("nvfp4_act_headroom: no NVFP4 dynamic-block input quantizer matched, so this is equivalent to "
+                      "plain max calibration. Check that the recipe enables NVFP4 activation quantizers.")
+    swapped = []
+    try:
+        for _, q in targets:
+            swapped.append((q, q._calibrator))
+            q._calibrator = NVFP4ActHeadroomCalibrator(q._num_bits, None, q._unsigned, block_size=16,
+                                                       anchor_percentile=cfg.anchor_percentile,
+                                                       upper_percentile=cfg.upper_percentile, rho=cfg.rho)
+        weight_fn(model, forward_loop, **weight_kw)
+    finally:
+        for q, original in swapped:
+            q._calibrator = original
 
 
 @torch.no_grad()
@@ -195,10 +243,17 @@ def mse_calibrate(model: nn.Module, forward_loop: Callable | None = None, distri
                 continue                                     # left at the max-calibrated amax (:717-718)
             # the sweep's candidates and losses do not depend on the FP8 normalization: a Four-Over-Six quantizer is
             # swept like any static NVFP4 one (NVFP4MSECalibrator, calib/mse.py:175-311) and normalizes by 256 after
-            best = ops.nvfp4_fp8_scale_sweep(m.weight.contiguous(), q._global_amax.reshape(1))
+            best = ops.nvfp4_fp8_scale_sweep(_pad_blocks16(m.weight), q._global_amax.reshape(1))
             q.amax = best.reshape(q._amax.shape)
             continue
         _mse_search_weight(m, step_size, start_multiplier, stop_multiplier)
+
+
+def _pad_blocks16(w):
+    """The weight in the static NVFP4 block layout the sweep searches: the last dim zero-padded to a multiple of 16, as
+    ``_process_for_blockquant`` pads it (zeros change no block amax and add no error)."""
+    rem = w.shape[-1] % 16
+    return (F.pad(w, (0, 16 - rem)) if rem else w).contiguous()
 
 
 def _mse_search_weight(m, step_size, start_multiplier, stop_multiplier):
@@ -267,7 +322,7 @@ def local_hessian_calibrate(model: nn.Module, forward_loop: Callable | None = No
         e = acc.get(id(q))
         hess = None if e is None or e[1] == 0 else e[0] / e[1]
         if fp8_scale_sweep and q.is_nvfp4_static:
-            best = ops.nvfp4_fp8_scale_sweep(m.weight.contiguous(), q._global_amax.reshape(1), hessian=hess)
+            best = ops.nvfp4_fp8_scale_sweep(_pad_blocks16(m.weight), q._global_amax.reshape(1), hessian=hess)
             q.amax = best.reshape(q._amax.shape)
         elif not fp8_scale_sweep and q._calibrator is not None:
             # the multiplier search (:720-728): under the Hessian metric where the forward reached this weight, else
@@ -810,7 +865,7 @@ def gptq(model: nn.Module, forward_loop: Callable | None = None, perc_damp: floa
         state[name] = None
 
 
-__all__ = ["max_calibrate", "mse_calibrate", "local_hessian_calibrate", "find_shared_weight_groups", "SHARED_PATTERNS", "smoothquant", "awq_lite", "awq_clip", "enable_stats_collection",
+__all__ = ["max_calibrate", "mse_calibrate", "local_hessian_calibrate", "nvfp4_act_headroom_calibrate", "find_shared_weight_groups", "SHARED_PATTERNS", "smoothquant", "awq_lite", "awq_clip", "enable_stats_collection",
            "gptq", "update_hessian", "compute_hessian_inverse", "gptq_blockwise_update",
            "gptq_blockwise_update_composed",
            "finish_stats_collection", "weight_only_quantize", "apply_pre_quant_scale_and_smooth",

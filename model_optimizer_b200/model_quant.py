@@ -69,6 +69,7 @@ def calibrate(model: nn.Module, algorithm="max", forward_loop: Callable | None =
         "mse": model_calib.mse_calibrate,
         "local_hessian": model_calib.local_hessian_calibrate,
         "gptq": model_calib.gptq,
+        "nvfp4_act_headroom": model_calib.nvfp4_act_headroom_calibrate,
     }.get(algorithm)
     if fn is None:
         raise ValueError(f"Unsupported calibration algorithm: {algorithm}")

@@ -240,6 +240,7 @@ class TensorTable:
         if fused and (ys is None or unit != "block16"):
             raise B200QuantError("a fused table needs outputs and unit='block16'")
         self.dtype = xs[0].dtype
+        self.unit = unit
         self.device = xs[0].device
         es = xs[0].element_size()
         per_cta = 1024 if unit == "vec32" else 512                 # amax: 256 thr x 4 vectors; NVFP4: 256 thr x 2 blocks
@@ -263,6 +264,7 @@ class TensorTable:
             first += (n_units + per_cta - 1) // per_cta
         self.total_ctas = first
         self.n = len(rows)
+        self.max_slot = max(r[4] for r in rows)
         self.table = torch.tensor(rows, dtype=torch.int64).to(self.device)
         self.live = None
         if fused:
@@ -420,6 +422,27 @@ def nvfp4_block_log2_hist_(hist: torch.Tensor, running_max: torch.Tensor, x: tor
         raise B200QuantError("last dim must be a multiple of 16 (pad with zeros first)")
     call("b200q_nvfp4_block_log2_hist", x.data_ptr(), _dt(x), x.numel() // 16, float(log2_min), float(log2_max),
          hist.numel(), hist.data_ptr(), running_max.data_ptr(), _stream(x))
+    return hist
+
+
+def nvfp4_block_log2_hist_multi_(hist: torch.Tensor, running_max: torch.Tensor, table: TensorTable,
+                                 log2_min: float = -40.0, log2_max: float = 40.0) -> torch.Tensor:
+    """``nvfp4_block_log2_hist_(hist[slot_i], running_max[slot_i : slot_i + 1], x_i)`` for every tensor of ``table``
+    (built with ``unit="block16"``) in ONE launch: ``hist`` is the int64 ``[n_slots, nbins]`` table, ``running_max``
+    the fp32 ``[n_slots]`` slots; entries that share a slot accumulate into it."""
+    _slots(running_max, "running_max")
+    if hist.dtype != torch.int64 or not hist.is_cuda or not hist.is_contiguous() or hist.dim() != 2:
+        raise B200QuantError("hist must be a contiguous int64 CUDA tensor [n_slots, nbins]")
+    if table.unit != "block16":
+        raise B200QuantError("the table must be built with unit='block16'")
+    if running_max.numel() != hist.shape[0] or table.max_slot >= hist.shape[0] or hist.device != table.device \
+            or running_max.device != table.device:
+        raise B200QuantError(f"hist / running_max must have a row per slot on {table.device} (largest slot "
+                             f"{table.max_slot}, {hist.shape[0]} rows)")
+    with torch.cuda.device(table.device):
+        call("b200q_nvfp4_block_log2_hist_multi", table.table.data_ptr(), table.n, table.total_ctas, _DT[table.dtype],
+             float(log2_min), float(log2_max), hist.shape[1], hist.data_ptr(), running_max.data_ptr(),
+             torch.cuda.current_stream(table.device).cuda_stream)
     return hist
 
 

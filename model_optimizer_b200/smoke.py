@@ -128,6 +128,15 @@ def run():
     fbest = ops.nvfp4_static_mse_sweep(x, torch.from_numpy(fa0).cuda(), torch.tensor([fg], device="cuda"), fmult, 256.0)
     fwant, _, _ = nvfp4_mse_oracle.search(xh, fa0, fg, fmult.cpu().numpy(), 256.0, "cuda")
     assert np.array_equal(fbest.cpu().numpy().view(np.uint32), fwant.view(np.uint32)), "Four-Over-Six search mismatch"
+    # (9) the grouped NVFP4 block log2 histogram against one per-tensor launch per entry (entries 0 and 2 share slot 0)
+    hx = [x, (x * 1e-3).contiguous(), x[:3].contiguous()]
+    hh, hm = torch.zeros(2, 512, dtype=torch.int64, device="cuda"), torch.zeros(2, dtype=torch.float32, device="cuda")
+    ops.nvfp4_block_log2_hist_multi_(hh, hm, ops.TensorTable(hx, [0, 1, 0], unit="block16"))
+    wh, wm = torch.zeros_like(hh), torch.zeros_like(hm)
+    for t, sl in zip(hx, (0, 1, 0)):
+        ops.nvfp4_block_log2_hist_(wh[sl], wm[sl:sl + 1], t)
+    assert torch.equal(hh, wh) and torch.equal(hm, wm), "grouped block log2 histogram mismatch"
     torch.cuda.synchronize()
     print("smoke ok: collect / fake quant (NVFP4, FP8, INT8) / pack (NVFP4, INT4) / grouped and fused launches / histogram + "
-          "amax searches / MSE sweep / Hadamard rotation / GPTQ block / Four-Over-Six search match the oracle")
+          "amax searches / MSE sweep / Hadamard rotation / GPTQ block / Four-Over-Six search / grouped block log2 "
+          "histogram match the oracle")
