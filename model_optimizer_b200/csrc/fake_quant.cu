@@ -49,72 +49,6 @@ struct IntParams {
   float max_bound, min_bound;
 };
 
-__device__ __forceinline__ float min_nan(float a, float b) {
-  float r;
-  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ float max_nan(float a, float b) {
-  float r;
-  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
-
-__device__ __noinline__ float int_fq_ref_noinline(float x, float scale, float maxb, float minb) {
-  float o = rintf(__fmul_rn(x, scale));
-  o = o > maxb ? maxb : o;
-  o = o < minb ? minb : o;
-  return __fdiv_rn(o, scale);
-}
-
-struct IntScale {
-  float scale, y, maxb, minb;
-  bool zero, fast;
-  __device__ __forceinline__ void setup(float amax, float max_bound, float min_bound) {
-    maxb = max_bound;
-    minb = min_bound;
-    zero = amax < (1.0f / (1 << 24));
-    scale = __fdiv_rn(max_bound, amax);
-    ExactDiv d(scale);
-    y = d.y;
-    // fast path: hoisted exact division + magic-number RNE (valid while |q| <= 2^21)
-    fast = d.ok && scale > 0.f && max_bound <= 2097152.0f;
-  }
-  // reference order (tensor_quant_gpu.cu:43-56), one element
-  __device__ __forceinline__ float apply_ref(float x) const {
-    if (zero) return 0.f;
-    float o = rintf(__fmul_rn(x, scale));
-    o = o > maxb ? maxb : o;
-    o = o < minb ? minb : o;
-    return __fdiv_rn(o, scale);
-  }
-  // same result, branch-free: rint via 1.5*2^23 (round-to-nearest-even of the FADD), NaN-keeping
-  // clamps, 3-FFMA exact division; the sign of a zero result comes from x*scale like rint's does
-  __device__ __forceinline__ float apply_fast(float x) const {
-    const float t = __fmul_rn(x, scale);
-    float o = __fadd_rn(__fadd_rn(t, 12582912.0f), -12582912.0f);
-    o = max_nan(min_nan(o, maxb), minb);
-    const float q = __fmul_rn(o, y);
-    const float r = __fmaf_rn(q, -scale, o);
-    return copysignf(__fmaf_rn(y, r, q), t);
-  }
-  template <int N> __device__ __forceinline__ void apply_vec(float *f) const {
-    if (zero) {
-#pragma unroll
-      for (int e = 0; e < N; ++e) f[e] = 0.f;
-    } else if (fast) {
-#pragma unroll
-      for (int e = 0; e < N; ++e) f[e] = apply_fast(f[e]);
-    } else {
-      // rare (scale outside the exact-division window / > 21-bit formats): out-of-line reference
-      // math, still fully unrolled so f[] stays in registers
-#pragma unroll
-      for (int e = 0; e < N; ++e) f[e] = int_fq_ref_noinline(f[e], scale, maxb, minb);
-    }
-  }
-  __device__ __forceinline__ float apply(float x) const { return apply_ref(x); }
-};
-
 // plain torch-style cast round trip (amax == None): overflow -> NaN
 __device__ __forceinline__ float fp8_torch_roundtrip(float v) {
   return e4m3_bits_to_f32(f32_to_e4m3fn_torch(v));
@@ -133,7 +67,7 @@ __global__ void __launch_bounds__(kEwThreads)
 
   pdl_launch_dependents();
   pdl_wait();
-  IntScale is;
+  IntQ is;
   Fp8Scale fs;
   if constexpr (MODE == kPerTensor && KIND != 2) {
     const float amax = load_scalar(ip.amax, ip.amax_dtype, 0);
@@ -181,17 +115,14 @@ __global__ void __launch_bounds__(kEwThreads)
           const float a1 = load_scalar(ip.amax, ip.amax_dtype, ((e0 + 1) / cm.outer) % cm.n_amax);
           if constexpr (KIND == 0) {
             is.setup(a0, ip.max_bound, ip.min_bound);
-            f[e] = is.apply(f[e]);
+            f[e] = is.apply_ref(f[e]);
             is.setup(a1, ip.max_bound, ip.min_bound);
-            f[e + 1] = is.apply(f[e + 1]);
+            f[e + 1] = is.apply_ref(f[e + 1]);
           } else {
             Fp8Scale s0, s1;
             s0.setup(a0, ip.max_bound != 0.f);
             s1.setup(a1, ip.max_bound != 0.f);
-            float lo, hi;
-            e4m3x2_to_f32x2(f32x2_to_e4m3x2(__fmul_rn(f[e], s0.scale), __fmul_rn(f[e + 1], s1.scale)), lo, hi);
-            f[e] = __fmul_rn(lo, s0.inv);
-            f[e + 1] = __fmul_rn(hi, s1.inv);
+            s0.apply2(f[e], f[e + 1], s1);
           }
         }
       } else if constexpr (KIND == 0) {
@@ -223,9 +154,9 @@ __global__ void __launch_bounds__(kEwThreads)
     } else {
       const float amax = load_scalar(ip.amax, ip.amax_dtype, n_amax == 1 ? 0 : (i / outer) % n_amax);
       if constexpr (KIND == 0) {
-        IntScale is;
+        IntQ is;
         is.setup(amax, ip.max_bound, ip.min_bound);
-        v = is.apply(v);
+        v = is.apply_ref(v);
       } else {
         Fp8Scale fs;
         fs.setup(amax, ip.max_bound != 0.f);

@@ -86,9 +86,7 @@ __global__ void __launch_bounds__(kGptqThreads) gptq_block_kernel(GptqArgs a) {
     if constexpr (FMT == kGptqNvfp4Static) {  // the lane's 4 columns lie in one 16-element block
       const float s = has_cols ? ss.block_scale(((const float *)a.amax)[r * a.amax_row_stride + (a.col0 + c_lo) / kBlk])
                                : 1.f;
-      // nvfp4_scalar_quant (nvfp4_quant.py:87-100): zero scale -> zero block; nan/inf scale -> 1
-      zero_st = (s == 0.0f);
-      s_st = (zero_st || !(fabsf(s) <= 3.4028234664e38f)) ? 1.0f : s;
+      s_st = static_block_scale_safe(s, zero_st);
     }
     const ExactDiv dst(s_st);
 
@@ -117,16 +115,12 @@ __global__ void __launch_bounds__(kGptqThreads) gptq_block_kernel(GptqArgs a) {
           if constexpr (FMT == kGptqInt) {
             q = iq[k].apply(x);
           } else if constexpr (FMT == kGptqFp8) {
-            float dummy = 0.f;
-            q = x;
-            fs[k].apply2(q, dummy);
+            q = fs[k].apply(x);
           } else if constexpr (FMT == kGptqNvfp4Static) {
-            const bool fast = mb < 0x7f800000u && s_st > 0.f && s_st >= 0x1p-40f && s_st <= 0x1p60f;
-            q = zero_st ? 0.f : qdq_e2m1_one(__fadd_rn(x, 0.f), s_st, dst, fast);
+            q = zero_st ? 0.f : qdq_e2m1_one(__fadd_rn(x, 0.f), dst, dst.block_ok(mb < 0x7f800000u));
           } else {
-            const float s = ds.block_scale(mn ? __uint_as_float(mn - 1u) : __uint_as_float(0x7fc00000u), d6);
-            const bool fast = mb < 0x7f800000u && s >= 0x1p-40f && s <= 0x1p60f;
-            q = qdq_e2m1_one(__fadd_rn(x, 0.f), s, ExactDiv(s), fast);
+            const ExactDiv d(ds.block_scale(mn ? __uint_as_float(mn - 1u) : __uint_as_float(0x7fc00000u), d6));
+            q = qdq_e2m1_one(__fadd_rn(x, 0.f), d, d.block_ok(mb < 0x7f800000u));
           }
           err = __fdiv_rn(__fsub_rn(x, q), s_u[i * sp + i]);
           qv[k] = q;

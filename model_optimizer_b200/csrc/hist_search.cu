@@ -111,18 +111,13 @@ __global__ void __launch_bounds__(kHsThreads)
   const int i = start_bin + (int)blockIdx.x * stride;
   const float amax = centers[i];
   IntQ q;
-  float sc = 0.f, inv = 0.f;
-  if (num_bits > 0) {
-    q.setup(amax, max_bound, min_bound);
-  } else {
-    const float safe = (amax <= (1.0f / (1 << 24))) ? 1.0f : amax;
-    sc = __fdiv_rn(448.0f, safe);
-    inv = __fdiv_rn(1.0f, sc);
-  }
+  Fp8Scale fs;
+  if (num_bits > 0) q.setup(amax, max_bound, min_bound);
+  else fs.setup(amax);
   double acc = 0.0;
   for (int idx = threadIdx.x; idx < n; idx += kHsThreads) {
     const float c = centers[idx];
-    const float qc = num_bits > 0 ? q.apply(c) : __fmul_rn(e4m3_round(__fmul_rn(c, sc)), inv);
+    const float qc = num_bits > 0 ? q.apply(c) : fs.apply(c);
     const float d = __fsub_rn(qc, c);
     acc += (double)__fmul_rn(__fmul_rn(d, d), (float)(long long)hist[idx]);
   }

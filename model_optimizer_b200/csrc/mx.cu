@@ -329,6 +329,12 @@ __device__ __forceinline__ int ceil_log2_clamped(float r) {
   return e > 127 ? 127 : e;
 }
 
+// one scaled element to its MXFP8 code: clamp to +-448 (NaN kept), then torch's e4m3fn cast
+__device__ __forceinline__ uint8_t mxfp8_cast(float v) {
+  if (v == v) v = fminf(fmaxf(v, -448.f), 448.f);
+  return f32_to_e4m3fn_torch(v);
+}
+
 template <typename Tag>
 __global__ void __launch_bounds__(kMxThreads)
     mxfp8_pack_kernel(const void *__restrict__ x, size_t n_rows, size_t row_len, size_t blocks_per_row,
@@ -364,11 +370,7 @@ __global__ void __launch_bounds__(kMxThreads)
         } else {
           w = 0;
 #pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            float v = __fmul_rn(f[e + k], sf);
-            if (v == v) v = fminf(fmaxf(v, -448.f), 448.f);
-            w |= (uint32_t)f32_to_e4m3fn_torch(v) << (8 * k);
-          }
+          for (int k = 0; k < 4; ++k) w |= (uint32_t)mxfp8_cast(__fmul_rn(f[e + k], sf)) << (8 * k);
         }
         out.r[j * 4 + e / 4] = w;
       }
@@ -392,11 +394,7 @@ __global__ void __launch_bounds__(kMxThreads)
   if (scale_in) byte = scale_in[t];
   else byte = ceil_log2_clamped(__fdiv_rn(amax, 448.f)) + 127;
   const float sf = pow2f(127 - byte);
-  for (int e = 0; e < cnt; ++e) {
-    float v = __fmul_rn(Elem<Tag>::load1(x, base + e), sf);
-    if (v == v) v = fminf(fmaxf(v, -448.f), 448.f);
-    q[base + e] = f32_to_e4m3fn_torch(v);
-  }
+  for (int e = 0; e < cnt; ++e) q[base + e] = mxfp8_cast(__fmul_rn(Elem<Tag>::load1(x, base + e), sf));
   if (!scale_in) scale_out[t] = (uint8_t)byte;
 }
 

@@ -22,6 +22,39 @@ constexpr int kNvThreads = 256;
 // ---------------------------------------------------------------------------------------------
 // dynamic fake quant
 // ---------------------------------------------------------------------------------------------
+// dynamic fake quant of the blocks base + u * stride (u < UNROLL) that are below n.  COLLECT: also returns their |x|
+// max as raw magnitude bits in the element's own format -- what amax_tensor_multi_kernel reduces, NaN payload included
+// (the block scale is the same either way: a non-finite block max gives the 448 clamp whatever its payload); 0 otherwise.
+template <typename Tag, int VB, int UNROLL, bool COLLECT>
+__device__ __forceinline__ uint32_t dyn_fq_blocks(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t base,
+                                                  size_t stride, size_t n, const DynScale &ds, const ExactDiv &d6) {
+  Block<Tag, VB> b[UNROLL];
+#pragma unroll
+  for (int u = 0; u < UNROLL; ++u) {
+    const size_t i = base + (size_t)u * stride;
+    if (i < n) b[u].load(x, i);
+  }
+  uint32_t amax = 0;
+#pragma unroll
+  for (int u = 0; u < UNROLL; ++u) {
+    const size_t i = base + (size_t)u * stride;
+    if (i >= n) continue;
+    uint32_t mb;
+    if constexpr (COLLECT) {
+      const uint32_t nb = b[u].prep_and_absmax_native_bits();
+      amax = max(amax, nb);
+      mb = Elem<Tag>::absbits_to_f32bits(nb);
+    } else {
+      mb = b[u].prep_and_absmax_bits();
+    }
+    const bool finite = mb < 0x7f800000u;
+    const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
+    qdq_block<Tag, VB>(b[u], s, finite);
+    b[u].store(y, i);
+  }
+  return amax;
+}
+
 template <typename Tag, int VB, int UNROLL>
 __global__ void __launch_bounds__(kNvThreads)
     nvfp4_dyn_kernel(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t n_blocks,
@@ -32,22 +65,7 @@ __global__ void __launch_bounds__(kNvThreads)
   ds.setup(load_scalar(gamax, gamax_dtype, 0));
   const ExactDiv d6(ds.six_gs);
   const size_t base = (size_t)blockIdx.x * (kNvThreads * UNROLL) + threadIdx.x;
-  Block<Tag, VB> b[UNROLL];
-#pragma unroll
-  for (int u = 0; u < UNROLL; ++u) {
-    const size_t i = base + (size_t)u * kNvThreads;
-    if (i < n_blocks) b[u].load(x, i);
-  }
-#pragma unroll
-  for (int u = 0; u < UNROLL; ++u) {
-    const size_t i = base + (size_t)u * kNvThreads;
-    if (i >= n_blocks) continue;
-    const uint32_t mb = b[u].prep_and_absmax_bits();
-    const bool finite = mb < 0x7f800000u;
-    const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
-    qdq_block<Tag, VB>(b[u], s, finite);
-    b[u].store(y, i);
-  }
+  dyn_fq_blocks<Tag, VB, UNROLL, false>(x, y, base, kNvThreads, n_blocks, ds, d6);
 }
 
 // TMA-store variant (north-star "TMA bulk staging" on the WRITE side; knob "nvfp4_tma_store"): the CTA's 16 KB of
@@ -92,40 +110,7 @@ __global__ void __launch_bounds__(kNvThreads)
   }
 }
 
-// dynamic fake quant of the blocks base + u * stride (u < UNROLL) that are below n.  COLLECT: also returns their |x|
-// max as raw magnitude bits in the element's own format -- what amax_tensor_multi_kernel reduces, NaN payload included
-// (the block scale is the same either way: a non-finite block max gives the 448 clamp whatever its payload); 0 otherwise.
-template <typename Tag, int VB, int UNROLL, bool COLLECT>
-__device__ __forceinline__ uint32_t dyn_fq_blocks(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t base,
-                                                  size_t stride, size_t n, const DynScale &ds, const ExactDiv &d6) {
-  Block<Tag, VB> b[UNROLL];
-#pragma unroll
-  for (int u = 0; u < UNROLL; ++u) {
-    const size_t i = base + (size_t)u * stride;
-    if (i < n) b[u].load(x, i);
-  }
-  uint32_t amax = 0;
-#pragma unroll
-  for (int u = 0; u < UNROLL; ++u) {
-    const size_t i = base + (size_t)u * stride;
-    if (i >= n) continue;
-    uint32_t mb;
-    if constexpr (COLLECT) {
-      const uint32_t nb = b[u].prep_and_absmax_native_bits();
-      amax = max(amax, nb);
-      mb = Elem<Tag>::absbits_to_f32bits(nb);
-    } else {
-      mb = b[u].prep_and_absmax_bits();
-    }
-    const bool finite = mb < 0x7f800000u;
-    const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
-    qdq_block<Tag, VB>(b[u], s, finite);
-    b[u].store(y, i);
-  }
-  return amax;
-}
-
-// the same kernel over a table of tensors (common.cuh MultiDesc): CTA -> (tensor, tile of 256 * UNROLL blocks);
+// nvfp4_dyn_kernel over a table of tensors (common.cuh MultiDesc): CTA -> (tensor, tile of 256 * UNROLL blocks);
 // each tensor's global amax is amax_base[slot] (the engine's flat _amax arena).
 // COLLECT: the pass is also the calibration collect -- the CTA's |x| max goes into the fp32 slot slots[slot] exactly as
 // amax_tensor_multi_kernel puts it there (unsigned atomic max on the bit pattern, nothing for an all-zero tile), so the
@@ -420,17 +405,15 @@ __device__ __forceinline__ uint2 encode_block(Block<Tag, VB> &b, float denom, bo
   // divided by denom must not round to zero -- a quotient that underflows to -0.0 loses the sign below, while the
   // reference's (-0.0 < 0) is false; such blocks take the explicit path
   constexpr float kMaxDenom = std::is_same<Tag, BF16Tag>::value ? 0x1p16f : (std::is_same<Tag, F16Tag>::value ? 0x1p60f : 1.0f);
-  const bool fast = finite && (denom >= 0x1p-40f) && (denom <= kMaxDenom);
+  const bool fast = d.block_ok(finite, kMaxDenom);
   if (fast) {
     // the correctly rounded quotient carries the sign the reference derives from (weight < 0): q = x * y has x's sign,
     // the residual only corrects its last bit, and for x = -0.0 the chain gives (+0) + (-0) = +0 -- sign bit clear,
     // exactly as (-0.0 < 0) is false.  So no sign fix-up and no -0.0 normalisation of the inputs is needed here.
 #pragma unroll
     for (int e = 0; e < kBlk; e += 2) {
-      const float q0 = __fmul_rn(f[e], d.y), q1 = __fmul_rn(f[e + 1], d.y);
-      const float t0 = __fmaf_rn(q0, -denom, f[e]), t1 = __fmaf_rn(q1, -denom, f[e + 1]);
-      const float a0 = __fmaf_rn(d.y, t0, q0);
-      const float a1 = __fmaf_rn(d.y, t1, q1);
+      float a0 = f[e], a1 = f[e + 1];
+      d.quot2(a0, a1);
       const uint32_t c = f32x2_to_e2m1x2(a0, a1) & 0xffu;  // byte = code[odd] << 4 | code[even]
       if (e < 8) lo |= c << (4 * e);
       else hi |= c << (4 * (e - 8));

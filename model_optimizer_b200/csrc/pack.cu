@@ -288,8 +288,7 @@ __global__ void __launch_bounds__(kPkThreads)
   if (fast) {
 #pragma unroll
     for (int e = 0; e < EPV; ++e) {
-      const float p = __fmul_rn(f[e], d.y);
-      float r = copysignf(__fmaf_rn(d.y, __fmaf_rn(p, -s0, f[e]), p), f[e]);
+      float r = copysignf(d.quot(f[e]), f[e]);
       if constexpr (ROUND_TO_T) r = E::round(r);
       f[e] = r;
     }
