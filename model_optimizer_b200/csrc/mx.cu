@@ -467,13 +467,15 @@ __global__ void __launch_bounds__(kMxThreads)
     const float inv = e >= 128 ? 0.f : pow2f(-e);
     Vec<16> out;
     if constexpr (Elem<Tag>::PER_WORD == 2) {
-      // 16-bit inputs: ONE FMA per element does the scaling and both fix-ups of the reference's rule
+      // 16-bit inputs: a multiply and an add per element do the scaling and both fix-ups of the reference's rule
       // (mxfp4_tensor.py:44-52: ties round DOWN, sign bit set unless y > 0) on top of the hardware RNE convert:
       //   * x * 2^-e has at most 11 significant bits, so multiplying by 2^-e * (1 - 2^-20) moves every value a few
       //     fp32 ulps towards zero: exact ties fall below their boundary, nothing else crosses one;
-      //   * adding -2^-149 (the smallest denormal) turns +0 (and a product that underflowed to +0) into a negative
-      //     zero-magnitude value -> code 8 like the reference's zeros, and leaves every other value's code alone
-      //     (2^-149 itself becomes +0 -> code 0, as y > 0 demands; normal values absorb it).
+      //   * adding -2^-149 (the smallest denormal) to the ROUNDED product turns +0 (and a product that underflowed to
+      //     +0) into a negative zero-magnitude value -> code 8 like the reference's zeros, and leaves every other
+      //     value's code alone (2^-149 itself becomes +0 -> code 0, as y > 0 demands; normal values absorb it).
+      //     One FMA would add it to the exact product instead: a bf16 product in (2^-150, 2^-149), which y rounds up
+      //     to 2^-149 > 0, would come out as -0 -> code 8.
       const float inv_t = __fmul_rn(inv, 1.0f - 0x1p-20f);
       const float neg_den = __uint_as_float(0x80000001u);
 #pragma unroll
@@ -485,7 +487,8 @@ __global__ void __launch_bounds__(kMxThreads)
           for (int k = 0; k < 4; ++k) {
             float lo, hi;
             Elem<Tag>::unpack(b[j].word(i + k), lo, hi);
-            w |= f32x2_to_e2m1x2(__fmaf_rn(lo, inv_t, neg_den), __fmaf_rn(hi, inv_t, neg_den)) << (8 * k);
+            w |= f32x2_to_e2m1x2(__fadd_rn(__fmul_rn(lo, inv_t), neg_den), __fadd_rn(__fmul_rn(hi, inv_t), neg_den))
+                 << (8 * k);
           }
           out.r[j * 2 + i / 4] = w;
         }

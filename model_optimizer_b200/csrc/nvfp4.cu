@@ -394,9 +394,10 @@ __device__ __noinline__ uint32_t encode_pair_slow(float x0, float x1, float deno
   return c0 | (c1 << 4);
 }
 
-// codes for the 16 elements of a block given the combined divisor denom = float(bs8) * s2
+// codes for the 16 elements of a block given the combined divisor denom = float(bs8) * s2; amax_b: the quant block's
+// |x| max (+inf / NaN for a non-finite block)
 template <typename Tag, int VB>
-__device__ __forceinline__ uint2 encode_block(Block<Tag, VB> &b, float denom, bool finite) {
+__device__ __forceinline__ uint2 encode_block(Block<Tag, VB> &b, float denom, float amax_b) {
   float f[kBlk];
   b.to_floats(f);
   uint32_t lo = 0, hi = 0;
@@ -405,7 +406,11 @@ __device__ __forceinline__ uint2 encode_block(Block<Tag, VB> &b, float denom, bo
   // divided by denom must not round to zero -- a quotient that underflows to -0.0 loses the sign below, while the
   // reference's (-0.0 < 0) is false; such blocks take the explicit path
   constexpr float kMaxDenom = std::is_same<Tag, BF16Tag>::value ? 0x1p16f : (std::is_same<Tag, F16Tag>::value ? 0x1p60f : 1.0f);
-  const bool fast = d.block_ok(finite, kMaxDenom);
+  // and no quotient may overflow: for x = -1e30 and denom = 5e-10, q = x * y = -inf, the residual is +inf and the
+  // correction fma(y, +inf, -inf) is NaN -- a code without x's sign, where the reference's -inf gives 0xF.  With
+  // |x| <= 2^126 * denom every q is finite (any |q| > 5 is code 7 whatever its last bits).  2^126 * denom is exact for
+  // denom in the window or overflows, hence the FLT_MAX cap: it keeps inf / NaN blocks on the explicit path
+  const bool fast = d.block_ok(amax_b <= fminf(__fmul_rn(0x1p126f, denom), 0x1.fffffep127f), kMaxDenom);
   if (fast) {
     // the correctly rounded quotient carries the sign the reference derives from (weight < 0): q = x * y has x's sign,
     // the residual only corrects its last bit, and for x = -0.0 the chain gives (+0) + (-0) = +0 -- sign bit clear,
@@ -467,7 +472,6 @@ __global__ void __launch_bounds__(kNvThreads)
     if (lg_l > 0)
       for (int o = 1; o < (1 << lg_l); o <<= 1) mb = max(mb, __shfl_xor_sync(0xffffffffu, mb, o));
     if (i >= n_blocks) continue;
-    const bool finite = mb < 0x7f800000u;
     float pbs;
     if constexpr (STATIC) {
       // nvfp4_tensor.py:139-161 + _cast_per_block_scale_to_fp8 (:32-48)
@@ -484,7 +488,7 @@ __global__ void __launch_bounds__(kNvThreads)
     const uint8_t bs8 = f32_to_e4m3fn_torch(pbs);
     if ((i & ((1u << lg_l) - 1u)) == 0) scales[i >> lg_l] = bs8;
     const float denom = __fmul_rn(e4m3_bits_to_f32(bs8), s2);
-    packed[i] = encode_block<Tag, VB>(b[u], denom, finite);
+    packed[i] = encode_block<Tag, VB>(b[u], denom, __uint_as_float(mb));
   }
 }
 

@@ -165,6 +165,24 @@ def reduce_amax(x, axis=None, keepdims=True):
                       np.abs(np.min(x, axis=axis, keepdims=keepdims))).astype(F32)
 
 
+def nan_skip_absmax(x, axis, keepdims=False):
+    """max |x| over ``axis`` skipping NaN elements, NaN where every element is NaN (fmaxf / tl.max).  Not
+    ``np.fmax.reduce``: its vectorized loops return NaN or a smaller element for some blocks holding signaling NaNs
+    (the fp32 images of bf16 NaN patterns with a clear quiet bit)."""
+    a = np.abs(np.asarray(x, dtype=F32))
+    nan = np.isnan(a)
+    m = np.max(np.where(nan, F32(0), a), axis=axis, keepdims=keepdims)
+    return np.where(np.all(nan, axis=axis, keepdims=keepdims), F32(np.nan), m).astype(F32)
+
+
+def canonical_nan(v):
+    """GPU fp32 arithmetic returns the canonical NaN 0x7fffffff (sign clear) whatever the NaN operand's sign; numpy on
+    the host keeps it.  Applied where the reference's tensor op (a CUDA op on a CUDA tensor) produces a NaN that a
+    sign-keeping cast then reads."""
+    v = np.asarray(v, dtype=F32)
+    return np.where(np.isnan(v), F32(np.nan), v).astype(F32)
+
+
 def reduce_block_amax(x, block):
     """core_utils.py:43-89 for block_sizes={-1: block}: [..., K] -> [..., K/block]."""
     x = np.asarray(x, dtype=F32)
@@ -354,8 +372,7 @@ def fake_quant_nvfp4(x, global_amax, dtype="bf16"):
     if pad:
         x2 = np.concatenate([x2, np.zeros((x2.shape[0], pad), dtype=F32)], axis=1)
     xb = x2.reshape(x2.shape[0], -1, 16)
-    with np.errstate(invalid="ignore"):                 # tl.max: NaN elements are skipped, an all-NaN block gives NaN
-        bmax = np.fmax.reduce(np.abs(xb), axis=2, keepdims=True)
+    bmax = nan_skip_absmax(xb, axis=2, keepdims=True)   # tl.max: NaN elements are skipped, an all-NaN block gives NaN
     s = nvfp4_block_scale_dynamic(bmax, global_amax)
     out = _nvfp4_qdq_with_scale(xb, s).reshape(x2.shape)[:, :k]
     return round_to(out.reshape(shape), dtype)
@@ -394,19 +411,22 @@ def fake_quant_nvfp4_static(x, block_amax, global_amax, quantize_block_scales=Tr
 # ------------------------------------------------------------------------------------------------
 # (3) quant and pack
 # ------------------------------------------------------------------------------------------------
-def pack_nvfp4(x, global_amax=None, block_amax=None, fp8_max_norm=448.0, block_size=16):
+def pack_nvfp4(x, global_amax=None, block_amax=None, fp8_max_norm=448.0, block_size=16, wsf2=None):
     """NVFP4QTensor.quantize (quantization/qtensor/nvfp4_tensor.py:253-342); static branch
-    (:139-161) when block_amax is given.  x last dim must be a multiple of block_size.
-    Returns (packed uint8 [..., K/2], scale bits uint8 [..., K/block_size], wsf2 float32)."""
+    (:139-161) when block_amax is given.  ``wsf2``: a caller-given weights_scaling_factor_2, used as is
+    (:281-282, get_weights_scaling_factor :169-202); global_amax is then not read.  x last dim must be a
+    multiple of block_size.  Returns (packed uint8 [..., K/2], scale bits uint8 [..., K/block_size], wsf2 float32)."""
     x = np.asarray(x, dtype=F32)
     k = x.shape[-1]
     xb = x.reshape(*x.shape[:-1], k // block_size, block_size)
-    if global_amax is None:
+    if wsf2 is not None and block_amax is not None:
+        raise ValueError("wsf2 and block_amax are mutually exclusive")
+    if global_amax is None and wsf2 is None:
         global_amax = reduce_amax(x)
-    g = F32(global_amax)
+    g = F32(0.0 if global_amax is None else global_amax)
     with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
         if block_amax is None:
-            s2 = F32(g / F32(6.0 * 448.0))
+            s2 = F32(wsf2) if wsf2 is not None else F32(g / F32(6.0 * 448.0))
             bmax = np.max(np.abs(xb), axis=-1)
             pbs = (bmax / F32(F32(6.0) * s2)).astype(F32)
             pbs = np.where(pbs == 0, F32(1.0), pbs)
@@ -513,7 +533,7 @@ def pack_fp8(x, scale, outer=1, x_dtype="bf16", scale_dtype="bf16", scale_is_0di
     s = _bcast_amax(x, scale, outer)
     res_dtype = x_dtype if (scale_dtype == x_dtype or scale_is_0dim) else "f32"
     with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
-        q = round_to((x / s).astype(F32), res_dtype)
+        q = canonical_nan(round_to((x / s).astype(F32), res_dtype))   # x / scale on the GPU: -NaN -> 0x7f
     _, bits = e4m3fn_torch_cast(q)
     return bits
 
@@ -876,7 +896,7 @@ def fake_quant_mx(x, block_size, fmt, dtype="bf16"):
     xp = np.concatenate([x, np.zeros((*x.shape[:-1], pad), F32)], axis=-1) if pad else x
     xb = xp.reshape(*x.shape[:-1], -1, block_size)
     with np.errstate(all="ignore"):
-        amax = np.fmax.reduce(np.abs(xb), axis=-1)
+        amax = nan_skip_absmax(xb, axis=-1)
         bad = (amax == 0) | np.isinf(amax) | np.isnan(amax)
         e = np.where(bad, 0, e8m0_exponent_nv(np.where(bad, F32(1), amax), fmt))
         scale = np.ldexp(F32(1), -e).astype(F32)[..., None]
@@ -915,7 +935,7 @@ def pack_mxfp8(x, scale_bytes=None):
             e = _ceil_log2_clamped((amax / F32(448.0)).astype(F32))
             scale_bytes = (e + 127).astype(np.uint8)
         sf = np.exp2(127.0 - scale_bytes.astype(np.float64)).astype(F32)
-        scaled = (xb * sf[..., None]).astype(F32)
+        scaled = canonical_nan((xb * sf[..., None]).astype(F32))     # x * 2^-e on the GPU: -NaN -> 0x7f
         scaled = np.where(np.isnan(scaled), scaled, np.clip(scaled, F32(-448.0), F32(448.0)))
     _, bits = e4m3fn_torch_cast(scaled)
     return bits.reshape(xp.shape)[..., :k], np.asarray(scale_bytes, dtype=np.uint8)

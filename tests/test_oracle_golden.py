@@ -113,6 +113,11 @@ def test_nvfp4_pack_and_qdq(golden):
         eq(sbits, golden[f"{k}/nvfp4_scales"])
         eq(np.float32(s2), golden[f"{k}/nvfp4_wsf2"])
         eq(o.unpack_nvfp4(packed, sbits, s2, _dt(k)), golden[f"{k}/nvfp4_deq"])
+        # the reference's own weights_scaling_factor_2, handed back to quantize: the same bytes and scales
+        p2, sb2, w2 = o.pack_nvfp4(x, global_amax=np.float32(1e30), wsf2=golden[f"{k}/nvfp4_wsf2"])
+        eq(p2, golden[f"{k}/nvfp4_packed"])
+        eq(sb2, golden[f"{k}/nvfp4_scales"])
+        eq(np.float32(w2), golden[f"{k}/nvfp4_wsf2"])
     assert n >= 6
 
 
