@@ -5,7 +5,9 @@
 // registers, the block amax is an in-register packed-integer max (no shuffles), the two-level
 // scale is computed once per block, E2M1 rounding is the reference's round-to-nearest-even, branch-free
 // (e2m1_round_mag / f32x2_to_e2m1x2 in common.cuh: sm_90 has no FP4 convert), and the block leaves with
-// one 32-byte vector store (fake quant) or one 8-byte + one 1-byte store (pack).
+// one 32-byte vector store (fake quant) or one 8-byte + one 1-byte store (pack).  The grouped dynamic fake quant
+// (nvfp4_dyn_multi_kernel) instead maps each whole tile of a 16-bit tensor lane-contiguously, two lanes per block
+// (dyn_fq_tile), so that every warp load and store fills whole 32-byte sectors.
 //
 // Reference semantics:
 //   dynamic fake quant : kernels/quantization/gemm/fp4_kernel_hopper.py:33-170 +
@@ -51,6 +53,46 @@ __device__ __forceinline__ uint32_t dyn_fq_blocks(const uint8_t *__restrict__ x,
     const float s = ds.block_scale(dyn_block_max(b[u], mb), d6);
     qdq_block<Tag, VB>(b[u], s, finite);
     b[u].store(y, i);
+  }
+  return amax;
+}
+
+// dyn_fq_blocks over the whole tile of kNvThreads * UNROLL blocks from block `tile`, 16-bit types, lane-contiguous: warp
+// w owns the tile's bytes [w, w + 1) * 32 * H * 16 and load i of lane l is the 16 bytes at i * 512 + l * 16 of them,
+// so each warp instruction covers 512 contiguous bytes (16 whole 32-byte sectors) where dyn_fq_blocks' covers half
+// of 32 sectors.  Lanes 2k and 2k + 1 hold the two halves of one block: each reduces its 8 elements, one shuffle
+// gives both lanes the block's |x| max, and each quantizes and stores its own half.  Same bits as dyn_fq_blocks,
+// and (COLLECT) the same CTA max of the returned values.
+template <typename Tag, int UNROLL, bool COLLECT>
+__device__ __forceinline__ uint32_t dyn_fq_tile(const uint8_t *__restrict__ x, uint8_t *__restrict__ y, size_t tile,
+                                                const DynScale &ds, const ExactDiv &d6) {
+  static_assert(Elem<Tag>::SIZE == 2, "a lane's 16 bytes are half a block only for 16-bit types");
+  constexpr int H = 2 * UNROLL;  // half blocks per lane
+  Block<Tag, 16, kBlk / 2> h[H];
+  // in half blocks (16 bytes): the tile starts at 2 * tile, warp w's bytes at 32 * H * w
+  const size_t h0 = 2 * tile + (size_t)(threadIdx.x >> 5) * (32 * H) + (threadIdx.x & 31);
+#pragma unroll
+  for (int i = 0; i < H; ++i) h[i].load(x, h0 + 32 * i);
+  // The stores mark their L2 lines evict-first: nothing reads the output back within the pass, and on an H100 the
+  // pass is 1.8 % faster than with default-priority stores (the hint on the loads made no difference; DESIGN §5).
+  const uint64_t pol = l2_evict_first_policy();
+  Vec<16> *dst = reinterpret_cast<Vec<16> *>(y) + h0;
+  uint32_t amax = 0;
+#pragma unroll
+  for (int i = 0; i < H; ++i) {
+    uint32_t mb;
+    if constexpr (COLLECT) {
+      const uint32_t nb = h[i].prep_and_absmax_native_bits();
+      amax = max(amax, nb);
+      mb = Elem<Tag>::absbits_to_f32bits(nb);
+    } else {
+      mb = h[i].prep_and_absmax_bits();
+    }
+    mb = max(mb, __shfl_xor_sync(0xffffffffu, mb, 1));
+    const bool finite = mb < 0x7f800000u;
+    const float s = ds.block_scale(dyn_pair_block_max(h[i], mb), d6);
+    qdq_block(h[i], s, finite);
+    stg(dst + 32 * i, h[i].v[0], pol);
   }
   return amax;
 }
@@ -111,7 +153,9 @@ __global__ void __launch_bounds__(kNvThreads)
 }
 
 // nvfp4_dyn_kernel over a table of tensors (common.cuh MultiDesc): CTA -> (tensor, tile of 256 * UNROLL blocks);
-// each tensor's global amax is amax_base[slot] (the engine's flat _amax arena).
+// each tensor's global amax is amax_base[slot] (the engine's flat _amax arena).  A whole tile of a 16-bit tensor goes
+// through dyn_fq_tile, the partial last tile of an entry (and every fp32 tile) through dyn_fq_blocks: the CTA owns the
+// same bytes either way.
 // COLLECT: the pass is also the calibration collect -- the CTA's |x| max goes into the fp32 slot slots[slot] exactly as
 // amax_tensor_multi_kernel puts it there (unsigned atomic max on the bit pattern, nothing for an all-zero tile), so the
 // slot ends bit-identical to that kernel's.  The atomic is skipped when the slot already holds at least that value:
@@ -126,8 +170,20 @@ __global__ void __launch_bounds__(kNvThreads, !COLLECT ? 0 : std::is_same<Tag, B
   DynScale ds;
   ds.setup(load_scalar(amax_base, gamax_dtype, (size_t)d.slot));
   const ExactDiv d6(ds.six_gs);
-  const size_t base = (size_t)(blockIdx.x - d.first_cta) * (kNvThreads * UNROLL) + threadIdx.x;
-  const uint32_t m = dyn_fq_blocks<Tag, VB, UNROLL, COLLECT>(d.x, d.y, base, kNvThreads, d.n_units, ds, d6);
+  const size_t tile = (size_t)(blockIdx.x - d.first_cta) * (kNvThreads * UNROLL);
+  uint32_t m = 0;
+  if constexpr (Elem<Tag>::SIZE == 2) {  // fp32 (64-byte blocks) keeps the per-block mapping
+    if (tile + kNvThreads * UNROLL <= d.n_units) {
+      m = dyn_fq_tile<Tag, UNROLL, COLLECT>(d.x, d.y, tile, ds, d6);
+    } else {  // the partial last tile of an entry, one block per thread at a time: no spills at 5 CTAs / SM
+#pragma unroll
+      for (int u = 0; u < UNROLL; ++u)
+        m = max(m, dyn_fq_blocks<Tag, VB, 1, COLLECT>(d.x, d.y, tile + u * kNvThreads + threadIdx.x, kNvThreads,
+                                                      d.n_units, ds, d6));
+    }
+  } else {
+    m = dyn_fq_blocks<Tag, VB, UNROLL, COLLECT>(d.x, d.y, tile + threadIdx.x, kNvThreads, d.n_units, ds, d6);
+  }
   if constexpr (COLLECT) {
     const uint32_t cm = block_max<kNvThreads>(m);
     if (threadIdx.x == 0 && cm != 0u) {
