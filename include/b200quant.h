@@ -144,7 +144,8 @@ int b200q_hist_search_mse(const float *hist, const float *centers, int n_centers
  * (calib/histogram.py:111-130) for a batch whose |x| max is *batch_amax: first batch -> range [0, x_max], nbins0 bins
  * (width = x_max / nbins0, the linspace step); later batches with x_max > upper -> nbins = ceil(x_max / width),
  * upper = last entry of arange(0, x_max + width, width).  A batch that would need more than `capacity` bins sets
- * `overflow` (the histogram buffer holds `capacity` floats) and later launches become no-ops.
+ * `overflow` = 1 (the histogram buffer holds `capacity` floats), a batch that would grow a zero-width range (an
+ * all-zero first batch) sets `overflow` = 2, and later launches become no-ops.
  * b200q_histogram_planned bins the batch with the planned (nbins, upper), adding into hist[0 .. nbins). */
 int b200q_hist_plan(const float *batch_amax, int nbins0, int capacity, void *plan_state, b200q_stream_t stream);
 int b200q_histogram_planned(const void *x, int dtype, size_t n, int take_abs, const void *plan_state,

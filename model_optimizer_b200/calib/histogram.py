@@ -66,6 +66,10 @@ class HistogramCalibrator(_Calibrator):
             self._host = {"upper": np.float32(f[0].item()), "width": np.float32(f[1].item()),
                           "xmax_grow": np.float32(f[2].item()), "nbins": int(p[3]), "init": int(p[4]),
                           "overflow": int(p[5]), "n_growths": int(p[6])}
+            if self._host["overflow"] == 2:
+                raise RuntimeError(
+                    "HistogramCalibrator: the first batch was all zeros, so the histogram range [0, 0] has zero width "
+                    "and cannot grow to a later batch's |x| max; collect a batch with a non-zero value first")
             if self._host["overflow"]:
                 raise RuntimeError(
                     f"HistogramCalibrator: a batch needed more than {self._capacity} bins (the range grew more than "
@@ -93,8 +97,11 @@ class HistogramCalibrator(_Calibrator):
             return None
         if h["n_growths"] == 0:
             return torch.linspace(0, float(h["upper"]), self._num_bins0 + 1).numpy()
+        # on the histogram's device, like the reference's arange(..., device=x.device): torch's CPU fp32 arange rounds
+        # some entries differently
         width = torch.tensor(h["width"])
-        return torch.arange(0, (torch.tensor(h["xmax_grow"]) + width).item(), width.item()).numpy()
+        return torch.arange(0, (torch.tensor(h["xmax_grow"]) + width).item(), width.item(),
+                            device=self._hist_buf.device).cpu().numpy()
 
     def compute_amax(self, method: str = "percentile", *, stride: int = 1, start_bin: int = 128,
                      percentile: float = 99.99):

@@ -6,6 +6,9 @@
 //   bin = (int)((v - min) * nbins / (max - min)) in fp32 with min = 0, bin == nbins -> nbins - 1,
 //   elements outside [min, max] (and NaN) are skipped.  The division by the (tensor-uniform) range
 //   uses the hoisted exact division, so the bin index is bit-identical to an IEEE divide.
+//   Two ranges where that formula has no usable value (DESIGN.md section 4, "Histogram ranges"): a zero range
+//   (max = 0) counts its zeros in bin nbins / 2 and skips every other value, and a product v * nbins that overflows
+//   fp32 (max above FLT_MAX / nbins) lands in the last bin.  Both only reach the exact-division fallback.
 // Counts are privatised per CTA in shared memory (u32 atomics) and flushed once with float
 // atomicAdd (histc returns float counts; integer-valued floats add exactly below 2^24).
 #include <cuda_fp16.h>
@@ -34,7 +37,8 @@ struct HistPlan {
   float xmax_grow;   // x_max of the batch that last grew the range (to rebuild the edges on the host)
   int nbins;         // current number of bins
   int initialized;
-  int overflow;      // a batch needed more than `capacity` bins: the histogram is no longer the reference's
+  int overflow;      // 1: a batch needed more than `capacity` bins; 2: a zero-width range had to grow.  Either way
+                     // the histogram is no longer the reference's, and later batches are not counted
   int n_growths;
   int reserved;
 };
@@ -54,7 +58,15 @@ __global__ void hist_plan_kernel(const float *__restrict__ batch_amax, int nbins
   }
   if (xmax > st->upper) {                                 // histogram.py:121
     const float width = st->width;
-    const int nb = (int)ceilf(__fdiv_rn(xmax, width));   // int((x_max / width).ceil().item())
+    if (!(width > 0.0f)) {                                // an all-zero first batch: a zero-width range cannot grow
+      st->overflow = 2;
+      return;
+    }
+    // int((x_max / width).ceil().item()).  Until the first growth the reference's edges come from linspace on the host,
+    // so width is a CPU scalar, and torch divides a device tensor by a CPU scalar as x_max * (1 / width); from then on
+    // its edges are a device arange and the division is a true one.
+    const float quot = st->n_growths == 0 ? __fmul_rn(xmax, __frcp_rn(width)) : __fdiv_rn(xmax, width);
+    const int nb = (int)ceilf(quot);
     if (nb > capacity || !(nb > 0)) {
       st->overflow = 1;
       return;
@@ -84,7 +96,9 @@ __device__ __forceinline__ void hist_put(float v, float vmax, float fbins, float
     const float p = __fmul_rn(t, y);
     q = __fmaf_rn(y, __fmaf_rn(p, -vmax, t), p);
   } else {
-    q = __fdiv_rn(t, vmax);
+    // a zero range counts its zeros in bin nbins / 2, as histc widens [0, 0] to [-1, 1]; a product v * nbins that
+    // overflows fp32 saturates to the last bin instead of wrapping to bin 0 (inf & 0x7fffff == 0)
+    q = vmax > 0.0f ? fminf(__fdiv_rn(t, vmax), fbins) : 0.5f * fbins;
   }
   int bin = (int)(__float_as_uint(__fadd_rz(q, 8388608.0f)) & 0x7fffffu);   // trunc(q), 0 <= q < 2^23
   bin = min(bin, last);
@@ -410,7 +424,8 @@ __global__ void __launch_bounds__(kPatThreads)
   auto add = [&](uint32_t m, uint32_t c) {                  // the exact histc bin of pattern m, once per pattern
     const float v = __uint_as_float(Elem<Tag>::absbits_to_f32bits(m));
     if (overflow || !(v >= 0.0f && v <= vmax)) return;      // NaN patterns and values above the range are skipped (histc)
-    const float q = __fdiv_rn(__fmul_rn(v, (float)nbins), vmax);
+    const float fbins = (float)nbins;                       // zero range and overflowing product: as in hist_put
+    const float q = vmax > 0.0f ? fminf(__fdiv_rn(__fmul_rn(v, fbins), vmax), fbins) : 0.5f * fbins;
     int bin = (int)(__float_as_uint(__fadd_rz(q, 8388608.0f)) & 0x7fffffu);
     bin = min(bin, nbins - 1);
     atomicAdd(hist + bin, (float)c);

@@ -98,7 +98,9 @@ def _check_scratch(scratch):
 def histogram_(hist: torch.Tensor, x: torch.Tensor, range_max: torch.Tensor, take_abs: bool = True,
                scratch: torch.Tensor | None = None) -> torch.Tensor:
     """hist[bin] += count with torch.histc(bins=hist.numel(), min=0, max=range_max) binning.  ``scratch``: see
-    ``histogram_planned_``."""
+    ``histogram_planned_``.  ``range_max == 0`` counts the zeros in bin ``nbins // 2``, where histc puts them when every
+    value is zero (it widens the empty range to [-1, 1]).  Non-zero values are outside [0, 0] and skipped; histc would
+    instead bin them over the data's own min and max, which this one-pass kernel does not know."""
     x = _prep(x, "x")
     _slots(hist, "hist")
     _slots(range_max, "range_max")

@@ -217,16 +217,32 @@ def histc(x, bins, vmax):
     (aten/src/ATen/native/cuda/SummaryOps.cu getBin, third party -- parity pinned only through
     tests/unit/torch/quantization/test_calibrator.py:141-181, exact counts vs numpy):
     bin = (int)((v - min) * bins / (max - min)) in fp32, bin == bins -> bins - 1, values outside
-    [min, max] dropped.  Counts returned as float32 like histc."""
+    [min, max] dropped.  Counts returned as float32 like histc.
+    A zero range is histc's: min = max = 0 takes the data's own min and max, and a range that is still empty is
+    widened by 1 on each side (all zeros: [-1, 1], the zeros in bin bins // 2).  A product v * bins that overflows fp32
+    (vmax above FLT_MAX / bins) has no value in that formula; it saturates to the last bin, as the kernels do
+    (DESIGN.md section 4, "Histogram ranges")."""
     x = np.asarray(x, dtype=F32).ravel()
-    vmax = F32(vmax)
-    keep = (x >= 0) & (x <= vmax)
-    v = x[keep]
-    with np.errstate(invalid="ignore", divide="ignore"):
-        b = ((v * F32(bins)) / vmax).astype(F32)
-    b = np.where(np.isfinite(b), b, 0).astype(np.int64)
+    lo, hi = F32(0), F32(vmax)
+    if hi == lo and x.size:
+        lo, hi = x.min(), x.max()
+    if hi == lo:
+        lo, hi = F32(lo - 1), F32(hi + 1)
+    keep = (x >= lo) & (x <= hi)
+    v = (x[keep] - lo).astype(F32)
+    with np.errstate(invalid="ignore", divide="ignore", over="ignore"):
+        b = ((v * F32(bins)).astype(F32) / (hi - lo)).astype(F32)
+    b = np.where(np.isnan(b), 0, np.minimum(b, F32(bins))).astype(np.int64)
     b = np.where(b == bins, bins - 1, b)
     return np.bincount(b, minlength=bins).astype(F32)
+
+
+def arange_f32(end, step):
+    """torch.arange(0, end, step) in fp32 as the device computes it: length ceil(end / step) in fp64, entry i the fp32
+    rounding of the exact product i * step.  np.arange(dtype=float32) and torch's CPU fp32 arange round some entries
+    differently."""
+    n = int(np.ceil(float(end) / float(step)))
+    return (np.arange(n, dtype=np.float64) * float(step)).astype(F32)
 
 
 class HistogramCalibrator:
@@ -236,6 +252,7 @@ class HistogramCalibrator:
         self.num_bins = num_bins
         self.hist = None
         self.edges = None
+        self.n_growths = 0
 
     def collect(self, x):
         x = np.asarray(x, dtype=F32)
@@ -248,8 +265,12 @@ class HistogramCalibrator:
         else:
             if x_max > self.edges[-1]:
                 width = self.edges[1] - self.edges[0]
-                self.num_bins = int(np.ceil(F32(x_max) / F32(width)))
-                self.edges = np.arange(0, F32(x_max) + F32(width), F32(width), dtype=F32)
+                # x_max / width on the device: before the first growth width is a host scalar (linspace edges), which
+                # torch applies as a multiplication by its fp32 reciprocal; later it is a device tensor
+                q = F32(x_max) * (F32(1) / F32(width)) if self.n_growths == 0 else F32(x_max) / F32(width)
+                self.num_bins = int(np.ceil(F32(q)))
+                self.edges = arange_f32(F32(x_max) + F32(width), width)
+                self.n_growths += 1
             h = histc(x, self.num_bins, self.edges[-1])
             h[: self.hist.size] += self.hist
             self.hist = h
